@@ -77,7 +77,7 @@ def make_pcm(n_chunks: int, seed: int) -> np.ndarray:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -281,6 +281,34 @@ def parity_vs_cpu(asr, eng, model, cpu) -> dict:
     }
 
 
+def dump_outputs(out_dir: str, hyps) -> None:
+    """What the timed path returned in its last step — one DecodeResult per chunk of this rank — as float64 arrays
+    under out_dir: tokens / times / tokens_confidence padded with -1 to the longest hypothesis, their lengths, and the
+    per-chunk score and confidence (well under 64 MB: 64 chunks x a few hundred tokens)."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(hyps)
+    L = max([len(h.tokens) for h in hyps] + [1])
+
+    def padded(get):
+        a = np.full((n, L), -1.0, dtype=np.float64)
+        for i, h in enumerate(hyps):
+            v = get(h)
+            if v is not None and len(v):
+                a[i, :len(v)] = np.asarray(list(v), dtype=np.float64)
+        return a
+
+    arrays = {
+        "tokens": padded(lambda h: h.tokens),
+        "token_lens": np.array([len(h.tokens) for h in hyps], dtype=np.float64),
+        "times": padded(lambda h: h.times),
+        "tokens_confidence": padded(lambda h: h.tokens_confidence),
+        "score": np.array([float(h.score) for h in hyps], dtype=np.float64),
+        "confidence": np.array([float(h.confidence or 0.0) for h in hyps], dtype=np.float64),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def _claim_stdout():
     """Only the JSON line may reach stdout: libraries (NCCL prints its version there) are redirected to stderr."""
     sys.stdout.flush()
@@ -314,6 +342,8 @@ def main():
                     help="after warm-up run ONE step between cudaProfilerStart/Stop and exit (for `ncu --profile-from-start off`)")
     ap.add_argument("--no-strong", action="store_true", help="skip the strong-scaling (configs[2]) record")
     ap.add_argument("--breakdown", action="store_true", help="print a per-stage wall-clock split (synchronised) to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's decode results (rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -471,7 +501,7 @@ def main():
     if sample_clocks:
         clocks.start()
     # one untimed step with the per-launch GEMM timing on: fills the library's event pool, so the timed region below does
-    # not create events (host time that showed up at N = 2, where the device-resident run measured slower than e2e)
+    # not create events (host time inside the timed region)
     lib.rvb_gemm_profile_begin()
     run_steps(1, False)
     lib.rvb_gemm_profile_end(None, None, None)
@@ -481,6 +511,8 @@ def main():
     gms, gfl, gn = C.c_double(), C.c_double(), C.c_longlong()
     lib.rvb_gemm_profile_end(C.byref(gms), C.byref(gfl), C.byref(gn))
     launches = launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, hyps)
     clk = clocks.stop() if sample_clocks else ({"sm_mhz": None, "sm_max_mhz": None, "reasons": ["not sampled"]} if rank == 0 else None)
     audio_s = args.chunks * 30.0 * args.steps * world
     value = audio_s / (ms / 1e3)
@@ -512,19 +544,9 @@ def main():
             peaks = json.load(f)
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet, dense BF16 (989 TFLOP/s at 700 W)"
     achieved_tf = (gfl.value / (gms.value / 1e3)) / 1e12 if gms.value > 0 else 0.0
-    # dram__bytes_read.sum + dram__bytes_write.sum per GEMM launch, from the committed ncu pass over one step of this
-    # same command (profiles/gemm_traffic.json, written from the ncu csv by tools/summarize_dram.py); None if absent
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "gemm_traffic.json")) as f:
-            tj = json.load(f)
-        if tj.get("shape") == args.shape and tj.get("chunks") == args.chunks:
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj.get("source")
-    except Exception:
-        pass
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -533,10 +555,9 @@ def main():
         "e2e": {"value": e2e_val, "unit": UNIT, "h2d_bytes_per_step": int(pcm_host.numel() * 2),
                 "d2h_bytes_per_step": int(d2h) + gather_bytes, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches),
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc2_kernel (2-CTA tcgen05 + TMA, all dense layers incl. conv2 implicit GEMM)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wg_kernel (wgmma + TMA, all dense layers incl. conv2 implicit GEMM)",
                      "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
-                     "peak_source": peak_src, "traffic": traffic, "traffic_unit": "DRAM bytes per launch (ncu)",
-                     "traffic_source": traffic_src,
+                     "peak_source": peak_src,
                      "launches_timed": int(gn.value), "kernel_ms_per_step": gms.value / args.steps,
                      "kernel_share_of_step": gms.value / ms if ms > 0 else None,
                      "algorithmic_flops_per_step": gfl.value / args.steps,
@@ -561,7 +582,7 @@ def main():
         try:
             line["parity"] = parity_vs_cpu(asr, eng, model, cpu)
             line["parity"]["mode"] = "bf16 (the timed configuration)"
-            # the same read-out in the fp32-accurate mode (precision="fp32": bf16x3 tcgen05 passes + fp32 attention)
+            # the same read-out in the fp32-accurate mode (precision="fp32": bf16x3 wgmma passes + fp32 attention)
             acc = reverb_b200.ReverbASR(os.path.join(mdir, "config.yaml"), os.path.join(mdir, "synth.pt"), gpu=local_rank,
                                         precision="fp32")
             line["parity_fp32_mode"] = parity_vs_cpu(acc, acc.engine, acc.model, cpu)

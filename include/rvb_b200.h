@@ -1,4 +1,4 @@
-/* reverb_b200 — C ABI of the B200-native hot path of revdotcom/reverb.
+/* reverb_b200 — C ABI of the H100-native hot path of revdotcom/reverb.
  *
  * The reference (100 % Python, asr/wenet) has no FFI of its own; this header is the boundary a maintainer binds
  * with ctypes (see INTEGRATION.md) to replace, one for one, the operator-level calls of the reference's hot path:
@@ -56,7 +56,7 @@ typedef struct rvb_model_config {
   int eos_id;           /* tokenizer_conf.special_tokens["<eos>"]; <= 0: vocab - 1 */
   int precision;        /* 0: bf16 tensor-core operands, fp32 accumulate (throughput mode, default)
                          * 1: "bf16x3" fp32-accurate mode — every GEMM operand is a (hi, lo) bf16 pair and runs as three
-                         *    tcgen05 passes hi.hi + lo.hi + hi.lo (~2^-16 relative), attention in fp32: for parity with
+                         *    wgmma passes hi.hi + lo.hi + hi.lo (~2^-16 relative), attention in fp32: for parity with
                          *    the reference's fp32 graph (bit-exact greedy ids); ~3x the tensor work */
 } rvb_model_config;
 
@@ -64,10 +64,10 @@ typedef struct rvb_model_config {
 RVB_API const char* rvb_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process */
 RVB_API unsigned long long rvb_launch_count(void);
-/* 0 = tcgen05/TMA GEMM (default), 1 = plain CUDA-core bring-up GEMM (debug only) */
+/* 0 = wgmma/TMA GEMM (default), 1 = plain CUDA-core bring-up GEMM (debug only), 2 = wgmma GEMM with 64-wide tiles */
 RVB_API int rvb_set_gemm_impl(int impl);
 RVB_API int rvb_get_gemm_impl(void);
-/* Per-launch CUDA-event timing of the tcgen05 GEMM kernel between begin/end (the roofline numbers of bench.py):
+/* Per-launch CUDA-event timing of the wgmma GEMM kernel between begin/end (the roofline numbers of bench.py):
  * total device time (ms), algorithmic FLOPs (2*M*N*K summed) and launch count.  end() synchronises. */
 RVB_API int rvb_gemm_profile_begin(void);
 RVB_API int rvb_gemm_profile_end(double* total_ms, double* total_flops, long long* launches);
@@ -215,7 +215,7 @@ RVB_API int rvb_decoder_step_logp(rvb_model* m, const float* d_enc_out, const in
 RVB_API int rvb_gemm_bf16(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act, int out_mode,
                   float alpha, void* d_out, int ldo, void* stream);
 /* The same GEMM in the fp32-accurate "bf16x3" mode (rvb_model_config.precision = 1): d_A (M, 2K) and d_W (N, 2K) hold
- * (hi | lo) bf16 pairs — hi = bf16(v), lo = bf16(v - hi), rvb_f32_to_bf16_pair builds them — and three tcgen05 passes
+ * (hi | lo) bf16 pairs — hi = bf16(v), lo = bf16(v - hi), rvb_f32_to_bf16_pair builds them — and three wgmma passes
  * hi.hi + lo.hi + hi.lo accumulate in fp32.  bf16 outputs (out_mode 0) are written as such a pair too: (M, 2N), or
  * (M, N) = (value half | residue half) of the N/2 GLU outputs; ldo = 0 selects that width. */
 RVB_API int rvb_gemm_bf16x3(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act, int out_mode,
@@ -236,7 +236,7 @@ RVB_API int rvb_attention(const void* d_q, const void* d_k, const void* d_v, con
                   const float* d_bias_v, void* d_out, int ldq, int ldk, int ldv, int ldp, int ldo, int Bq, int Tq, int Tk,
                   int H, int dk, int q_per_kv, const int* d_k_lens, const int* d_q_lens, int causal, float scale,
                   void* stream);
-/* tcgen05 attention (d_k = 64): group g owns query rows [g*Tq, ..) and key rows [g*Tk, ..); pointers address head 0;
+/* wgmma attention (d_k = 64): group g owns query rows [g*Tq, ..) and key rows [g*Tk, ..); pointers address head 0;
  * d_key_bias (groups, H, Tk) fp32 optional (added to q.k before scaling), d_k_lens (groups) optional; causal != 0
  * (needs Tq == Tk): key j is visible to query i iff j <= i (decoder self-attention, utils/mask.py subsequent_mask). */
 RVB_API int rvb_attention_tc(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk, int ldv,

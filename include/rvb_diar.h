@@ -1,7 +1,7 @@
 /* rvb_diar.h — C ABI of the diarization forward in librvb_b200.so (SURVEY.md §8f rank 1).
  *
  * The reference runs the two networks below through `pyannote.audio==3.3.1`
- * (/root/reference/diarization/infer_pyannote3.0.py:14,33-40: `Pipeline.from_pretrained(...)`, `pipeline(audio)`;
+ * (reference: diarization/infer_pyannote3.0.py:14,33-40: `Pipeline.from_pretrained(...)`, `pipeline(audio)`;
  * requirements.txt:1).  There is no FFI in the reference for this path; these are the entry points a binding of
  * `pyannote.audio.Model.__call__` for the segmentation / embedding models would replace:
  *

@@ -2,8 +2,8 @@
 
 ** parity unpinned **  The reference runs `pyannote.audio==3.3.1` behind
 `Pipeline.from_pretrained('Revai/reverb-diarization-v1')` (diarization/infer_pyannote3.0.py:14,33-40;
-diarization/requirements.txt:1).  Neither the package, its source nor the model weights exist in this image or under
-/root/reference, and the reference holds no tests or golden vectors for this path.  This file restates the PUBLISHED
+diarization/requirements.txt:1).  Neither the package, its source nor the model weights are available offline or in
+the reference repository, and the reference holds no tests or golden vectors for this path.  This file restates the PUBLISHED
 architecture of that pipeline's two networks from the upstream project's public description:
 
   * segmentation  `PyanNet`  (pyannote/audio/models/segmentation/PyanNet.py, v3.3.1): SincNet front-end

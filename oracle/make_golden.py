@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.npz|json by running the LIVE reference (/root/reference) in the
-authoring container.  Test infrastructure; run as `python -m oracle.make_golden`.
+"""Generate tests/golden/*.npz|json by running the LIVE reference (a revdotcom/reverb checkout named by
+RVB_REFERENCE_ROOT, oracle/refimport.py).  Test infrastructure; run as `python -m oracle.make_golden`.
 
-The Python reference cannot travel to the GPU box, so its outputs on seeded synthetic
+The tests must not depend on the Python reference, so its outputs on seeded synthetic
 inputs are committed as small fixtures.  Inputs (model weights, audio) are regenerated
 deterministically from seeds by reverb_b200/synth.py; a checksum of the weights is stored
 so that a drifted generator is detected instead of silently compared.

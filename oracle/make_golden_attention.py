@@ -1,5 +1,5 @@
 """ORACLE tooling (test infrastructure): pins the `attention` decode mode (autoregressive beam search with the left
-decoder, asr/wenet/transformer/search.py:251-360) against the LIVE reference in the authoring container.
+decoder, asr/wenet/transformer/search.py:251-360) against the LIVE reference (a reference checkout, see oracle/refimport.py).
 
 Re-creates the two synthetic models of tests/golden/{causal_ln,sym_bn}.json from their stored seeds, runs the
 reference's ASRModel.decode(['attention'], ...) batch by batch (two length penalties) and stores the token ids in

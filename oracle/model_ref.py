@@ -6,9 +6,9 @@ tensor ops over a flat state_dict, of the reference's model graph on the hot pat
   n-best -> (LSL) bi-transformer decoder, teacher forced -> log_softmax
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference/asr/wenet).  Pinned against the LIVE reference run in the authoring
-container (oracle/make_golden.py -> tests/golden/*.npz; tests/test_oracle_vs_reference.py
-re-checks whenever /root/reference is present).  The reference has no tests of its own
+the reference's asr/wenet).  Pinned against outputs of the LIVE reference
+(oracle/make_golden.py, make_golden_pins.py -> tests/golden/; checked by tests/test_oracle_golden.py and
+tests/test_oracle_vs_reference.py).  The reference has no tests of its own
 for this path (SURVEY.md §4), so "parity unpinned" by reference-held golden vectors;
 pinned instead by outputs of the reference itself.
 
@@ -92,7 +92,7 @@ def rel_attention(x, mask, pos_emb, sd: SD, p: str, H: int):
     v = _q(_lin(x, sd, p + ".linear_v")).view(B, T, H, dk).transpose(1, 2)
     pp = _q(F.linear(_q(pos_emb), _q(sd[p + ".linear_pos.weight"]))).view(1, -1, H, dk).transpose(1, 2)
     if EMULATE_BF16:
-        # the tcgen05 attention folds the position term: s = q.(k + p) + (u.k + v.p), with K'' = bf16(k + p)
+        # the wgmma attention folds the position term: s = q.(k + p) + (u.k + v.p), with K'' = bf16(k + p)
         kpp = _q(k + pp)
         cb = (sd[p + ".pos_bias_u"].unsqueeze(1) * k).sum(-1) + (sd[p + ".pos_bias_v"].unsqueeze(1) * pp).sum(-1)
         scores = (torch.matmul(q.transpose(1, 2), kpp.transpose(-2, -1)) + cb.unsqueeze(-2)) / math.sqrt(dk)

@@ -4,8 +4,8 @@ the restated pieces (fbank_np, model_ref, search_ref) — the CPU twin of the re
 asr/wenet/transformer/asr_model.py:331-432).
 
 Used (a) as the checker in tests/ and __graft_entry__.smoke(), (b) as the timed CPU
-baseline / `--impl reference` arm of bench.py (the Python reference itself cannot travel
-to the GPU box).  It executes the same ATen CPU operators as the reference does
+baseline / `--impl reference` arm of bench.py (the tests and the benchmark do not need the
+Python reference itself).  It executes the same ATen CPU operators as the reference does
 (conv2d / linear / matmul / softmax / layer_norm), so its timing is representative.
 """
 from __future__ import annotations

@@ -1,9 +1,9 @@
-"""Import the LIVE reference (revdotcom/reverb, /root/reference/asr) inside the
-authoring container so it can serve as the parity oracle's ground truth.
+"""Import the LIVE reference (a revdotcom/reverb checkout, $RVB_REFERENCE_ROOT/asr) so it can serve as the parity
+oracle's ground truth when the golden fixtures are (re)generated.
 
 TEST INFRASTRUCTURE ONLY.  Nothing in the product path (reverb_b200/) may import
-this module.  It only works where /root/reference exists (the authoring
-container); the GPU box uses the committed fixtures under tests/golden/.
+this module.  It only works where RVB_REFERENCE_ROOT points at a reference
+checkout; the test suite uses the committed fixtures under tests/golden/.
 
 Shims (SURVEY.md Appendix B):
   1. stub `whisper.tokenizer.LANGUAGES` (reference: asr/wenet/utils/common.py:23)
@@ -20,7 +20,7 @@ import wave
 import numpy as np
 import torch
 
-REFERENCE_ROOT = os.environ.get("RVB_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("RVB_REFERENCE_ROOT", "")
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -42,9 +42,10 @@ def _wave_load(path, normalize=False, **_kw):
 
 
 def import_reference():
-    """Returns the reference's `wenet` package (imported from /root/reference/asr)."""
+    """Returns the reference's `wenet` package (imported from asr)."""
     if not available():
-        raise RuntimeError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise RuntimeError("reference tree not found: set RVB_REFERENCE_ROOT to a revdotcom/reverb checkout (now %r)"
+                           % REFERENCE_ROOT)
     stub_dir = os.path.join(_HERE, "_stubs")
     ref_asr = os.path.join(REFERENCE_ROOT, "asr")
     # The repo root ships a drop-in `wenet` alias; make sure the reference wins here.

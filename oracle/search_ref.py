@@ -4,7 +4,7 @@ numpy/torch fp32 log-prob arrays.  Float semantics follow the reference: prefix 
 Python floats (C doubles) built from fp32 log-probs (`.item()`), rescoring scores are
 accumulated in fp32 (0-d torch tensors).
 
-Pinned against the LIVE reference in the authoring container (oracle/make_golden.py,
+Pinned against the LIVE reference (fixtures recorded by oracle/make_golden.py, checked by
 tests/test_oracle_vs_reference.py); the reference itself holds no tests (SURVEY.md §4).
 """
 from __future__ import annotations

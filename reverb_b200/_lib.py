@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI declared in include/rvb_b200.h (librvb_b200.so, sm_100a).
+"""ctypes binding of the C ABI declared in include/rvb_b200.h (librvb_b200.so, sm_90a).
 
 This is the only place the Python host code touches native code.  There is no CPU
 fallback: if the shared library is missing or a call fails, a RuntimeError is raised.

@@ -10,7 +10,7 @@
 //
 // Scores are never materialised in HBM (the reference writes (B,H,T',T') fp32 = 2.29 GB per layer at B=64).
 // Round-1 implementation: bf16 mma.sync.m16n8k16 with fp32 accumulation, online softmax in registers, K/V/P tiles
-// double-buffered through shared memory with cp.async.  (A tcgen05/TMEM version is the planned upgrade.)
+// double-buffered through shared memory with cp.async.  (attention_tc.cu is the wgmma version.)
 #include "kernels.h"
 
 namespace rvb {

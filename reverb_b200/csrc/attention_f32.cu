@@ -1,12 +1,12 @@
 // reverb_b200 — fp32 attention of the ACCURATE ("bf16x3") precision mode.
 //
 // In that mode every activation is a bf16 pair (hi, lo) with v = hi + lo to ~16 mantissa bits (GemmArgs::x3, kernels.h)
-// and the projections run as three tcgen05 passes.  The attention itself is only ~5 % of the encoder FLOPs, so here it
+// and the projections run as three wgmma passes.  The attention itself is only ~5 % of the encoder FLOPs, so here it
 // is evaluated directly in fp32 on the CUDA cores, operation for operation like the reference
 // (asr/wenet/transformer/attention.py:344-399 rel-pos, :102-127 forward_attention; decoder: MultiHeadedAttention):
 //     s[i,j] = ((q_i + u) . k_j + (q_i + v) . p_j) / sqrt(d_k)      (p: absolute key position, no rel_shift)
 //     s[mask == 0] = -inf ; a = softmax_j(s) ; a[mask == 0] = 0 ; o_i = sum_j a[i,j] v_j
-// The throughput path is attention_tc.cu (tcgen05, bf16 operands); this kernel exists so that a whole decode can be
+// The throughput path is attention_tc.cu (wgmma, bf16 operands); this kernel exists so that a whole decode can be
 // run at fp32-level accuracy for parity with the reference (token ids bit-exact, logits to ~1e-4).
 // One warp per query row; the row's scores live in shared memory.
 #include <math.h>

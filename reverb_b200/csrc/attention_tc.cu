@@ -1,23 +1,19 @@
-// reverb_b200 — tcgen05 / TMEM / TMA attention for the long (encoder self-attention, decoder source-attention) cases.
+// reverb_b200 — wgmma / TMA attention for the long (encoder self-attention, decoder source-attention) cases, sm_90a.
 //
 // Rel-pos scores without the second product.  The reference computes (asr/wenet/transformer/attention.py:378-397)
 //     s[i,j] = ((q_i + u) . k_j + (q_i + v) . p_j) / sqrt(d_k)          (p_j: ABSOLUTE key position, no rel_shift)
 // which is algebraically
 //     s[i,j] = ( q_i . (k_j + p_j)  +  (u . k_j + v . p_j) ) / sqrt(d_k) =  ( q_i . K''_j + c_j ) / sqrt(d_k)
-// so a small pre-kernel builds K'' = k + p (bf16) and the per-key bias c (fp32) once per layer, and the attention
-// itself is ONE tensor-core product per key tile plus a key bias: half the QK FLOPs and no P tiles.
+// so a small pre-kernel (or the projection GEMM's epilogue) builds K'' = k + p (bf16) and the per-key bias c (fp32)
+// once per layer, and the attention itself is ONE tensor-core product per key tile plus a key bias.
 //
-// Kernel (one CTA = 128 query rows of one (group, head); 2 CTAs / SM):
-//   warp 4 / lane 0 : TMA producer (Q once, K'' tiles double-buffered, V tiles) + tcgen05.mma issuer
-//                     S[128 x 128] = Q . K''^T  (M=128, N=128, 4 x K=16)         -> TMEM columns [0,128)
-//                     O[128 x  64] += P~ . V    (M=128, N=64, 8 x K=16, V as MN-major B) -> TMEM columns [128,192)
-//   warps 0..3      : one thread per query row: tcgen05.ld of its S row, mask + key bias, exp2, row sum, P~ written
-//                     to shared memory in the SWIZZLE_128B K-major layout the PV product reads as its A operand.
-// ONE pass over the key tiles with a lazily updated running maximum: P~ = exp2(s - m) uses the maximum m of the tiles
-// seen so far and m is only raised — with a rescale of the row sum and of the O accumulator in TMEM (tcgen05.ld /
-// scale / tcgen05.st by the row's own thread) — when a tile exceeds it by more than 2^8; until then P~ <= 256, well
-// inside bf16 / fp32 range, and O / row_sum is unchanged mathematically.  Rescales are rare after the first tile, so
-// S is computed once and the exponentials are the only per-element cost.  Scores / probabilities never touch HBM.
+// Kernel (one CTA = 128 query rows of one (group, head), 288 threads):
+//   warp 8 / lane 0 : TMA producer — Q once, then K'' and V tiles of 64 keys through AT_ST-deep rings
+//   warps 0..7      : two consumer warpgroups of 64 query rows each; per key tile
+//                       S[64 x 64]  = Q . K''^T        wgmma m64n64k16 x 4, both operands from shared memory
+//                       online softmax on the S fragments in registers (scale, key bias, masks, running max / sum)
+//                       O[64 x 64] += P~ . V           wgmma m64n64k16 x 4, P~ (bf16) from registers, V MN-major
+// Scores / probabilities never touch shared memory or HBM.
 #include <cuda.h>
 #include <math.h>
 #include <stdlib.h>
@@ -29,59 +25,18 @@
 namespace rvb {
 
 constexpr int AT_BM = 128;  // query rows per CTA
+constexpr int AT_BN = 64;   // keys per tile
 constexpr int AT_DK = 64;
-constexpr int AT_KST = 4;   // K'' stages
-constexpr int AT_VST = 3;   // V stages
-constexpr int AT_NS = 3;    // S accumulator buffers in TMEM: QK runs three tiles ahead of the softmax warps
-constexpr uint32_t AT_Q_BYTES = 128 * AT_DK * 2;  // 16 KB Q tile (= one 64-key K-block of P~)
-constexpr bool AT_TRUNC_P = true;                 // P~ truncated (ALU) instead of rounded (XU) to bf16, see the softmax loop
-
-// BN = keys per tile.  BN = 64: 2 CTAs / SM (TMEM 256 columns each) hide each other's barrier round trips;
-// BN = 128: 1 CTA / SM (512 columns).
-template <int BN>
-struct AtCfg {
-  static constexpr uint32_t KV_BYTES = BN * AT_DK * 2;   // one K'' / V tile
-  static constexpr uint32_t P_BYTES = 128 * BN * 2;      // P~: 128 rows x BN keys (BN / 64 K-blocks of 16 KB)
-  static constexpr uint32_t SMEM_FIXED = AT_Q_BYTES + (AT_KST + AT_VST) * KV_BYTES + 2 * P_BYTES + 1024 + 256;
-  static constexpr uint32_t TMEM_COLS = (BN == 128) ? 512 : 256;  // S0 [0,BN), S1 [BN,2BN), O [2BN,2BN+64), S2 [2BN+64,3BN+64)
-  static constexpr int CTAS_PER_SM = (BN == 128) ? 1 : 2;
-};
+constexpr int AT_ST = 4;    // K'' / V ring stages
+constexpr int AT_THREADS = 288;
+constexpr uint32_t AT_Q_BYTES = AT_BM * AT_DK * 2;     // 16 KB
+constexpr uint32_t AT_TILE_BYTES = AT_BN * AT_DK * 2;  // 8 KB
+constexpr uint32_t AT_SMEM_FIXED = AT_Q_BYTES + 2 * AT_ST * AT_TILE_BYTES + 256 /*barriers*/ + 1024 /*align slack*/;
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// Blackwell FMNMX3: max of three in one ALU instruction (halves the instruction count of the row maximum)
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-
-// 2^x for a PAIR of arguments on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f, |f| <= 1/2, degree-3
-// minimax polynomial for 2^f (max relative error 7.5e-5, far below the bf16 quantisation of P~), 2^n through the exponent
-// field.  x is clamped at -126 (2^-126 ~ 1e-38 underflows to nothing in the sums).  Used for a FRACTION of the
-// exponentials of interior tiles so that MUFU.EX2 (XU pipe, 16 / clk / SM) is not the only unit doing them.
-__device__ __forceinline__ float2 exp2_poly2(float2 x) {
-  const float2 magic = make_float2(12582912.f, 12582912.f), one2 = make_float2(1.f, 1.f);
-  x.x = fmaxf(x.x, -126.f);
-  x.y = fmaxf(x.y, -126.f);
-  const float2 xf = ffma2(x, one2, magic);                                   // n in the low mantissa bits
-  const float2 n = ffma2(xf, one2, make_float2(-12582912.f, -12582912.f));
-  const float2 f = ffma2(n, make_float2(-1.f, -1.f), x);
-  float2 p = ffma2(f, make_float2(0.05517164617776871f, 0.05517164617776871f), make_float2(0.2426111251115799f, 0.2426111251115799f));
-  p = ffma2(p, f, make_float2(0.6932609677314758f, 0.6932609677314758f));
-  p = ffma2(p, f, make_float2(0.9999280571937561f, 0.9999280571937561f));
-  return make_float2(__uint_as_float(__float_as_uint(p.x) + (__float_as_uint(xf.x) << 23)),
-                     __uint_as_float(__float_as_uint(p.y) + (__float_as_uint(xf.y) << 23)));
-}
-
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
 }
 
 struct AttnTcParams {
@@ -95,77 +50,25 @@ struct AttnTcParams {
   int left;    // number of left chunks, < 0 = all
   const uint32_t* key_bits;  // optional per-(query row, key) visibility bits (AttnTcArgs::key_bits)
   int bits_ld;
-  int pipe;    // 1: pull S(j+1) inside tile j's exponential loop (RVB_ATTN_PIPE=0 disables)
   float scale_log2;
 };
 
-// Pipeline (SW softmax warps + 1 control warp per CTA):
-//   control thread (warp SW, lane 0): TMA loads (Q, K'' x AT_KST stages, V x2) and all tcgen05.mma issue; S has AT_NS
-//     buffers in TMEM so QK(i+AT_NS) is queued while the softmax warps consume S(i); P~ is double-buffered in shared
-//     memory so PV(j) runs while P~(j+1) is produced.
-//   softmax warps (thread = query row): tile max, lazy running-max update, exp2 / row sum / P~.
-//     SW = 4 (default): one thread per row.  SW = 8 (RVB_ATTN_SW=8): warps w and w+4 share the 32 rows of TMEM lane quarter w%4 and
-//     each takes half of the tile's columns (and half of the O columns in the rescale / epilogue); the two partial
-//     tile maxima / row sums meet through shared memory and a 64-thread named barrier.  Measured slightly SLOWER than
-//     SW = 4 (0.403 vs 0.388 ms per encoder layer): the kernel is not short of warps; what bounds it is the
-//     ex2 + issue budget per tile and the per-tile hand-offs, which the split duplicates.
-// CW3: the control work is split over THREE warps — TMA loader, QK issuer, PV issuer (+ one idle warp so that the control
-// side is a whole warpgroup for setmaxnreg) — instead of one thread doing all three in turn.  Measured with the timing
-// ablations below: with the entire softmax arithmetic removed the kernel still took 0.43 ms per encoder layer, i.e. the
-// single control thread's chain of ~24 long-latency special instructions per tile (6 mbarrier waits, 8 tcgen05.mma,
-// 4 commits, 2 TMA issues, ...) was the critical path, not MUFU / issue slots / TMEM loads.
-// PT: P~ lives in TENSOR MEMORY instead of shared memory.  ncu showed the tensor sub-pipe occupied 75 % of the time at 15 %
-// of its FLOP rate: the N = 64 products are operand-fetch (shared-memory bandwidth) bound — per 64-key tile the MMAs read
-// Q 16 KB + K'' 8 KB + P~ 16 KB + V 8 KB next to 16 KB of P~ stores and 16 KB of TMA writes.  With PT the softmax thread
-// writes its packed P~ row over its own S row (tcgen05.st, 32 columns) and the PV product takes A from TMEM: 32 KB less
-// shared-memory traffic per tile, no proxy fence, and the S buffer returns to the QK issuer when PV(j) retires.
-template <int BN, int SW, int POLY, bool CW3 = false, bool PT = false>
-__global__ void __launch_bounds__(32 * (SW + (CW3 ? 4 : 1)), AtCfg<BN>::CTAS_PER_SM)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  using Cfg = AtCfg<BN>;
-  constexpr int AT_BN = BN;
-  constexpr uint32_t AT_TILE_BYTES = Cfg::KV_BYTES;
-  constexpr uint32_t AT_P_BYTES = Cfg::P_BYTES;
-  constexpr uint32_t AT_TMEM_COLS = Cfg::TMEM_COLS;
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + AT_Q_BYTES;               // AT_KST stages
-  uint8_t* sV = sK + AT_KST * AT_TILE_BYTES;   // AT_VST stages
-  uint8_t* sP = sV + AT_VST * AT_TILE_BYTES;        // 2 buffers x (BN / 64 K-blocks of 64 keys)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * AT_P_BYTES);
-  uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;                      // [AT_KST]
-  uint64_t* k_empty = k_full + AT_KST;              // [AT_KST]
-  uint64_t* v_full = k_empty + AT_KST;              // [AT_VST]
-  uint64_t* v_empty = v_full + AT_VST;              // [AT_VST]
-  uint64_t* s_full = v_empty + AT_VST;              // [AT_NS]
-  uint64_t* s_empty = s_full + AT_NS;               // [AT_NS]
-  uint64_t* p_full = s_empty + AT_NS;               // [2]
-  uint64_t* p_empty = p_full + 2;                   // [2]
-  uint64_t* o_done = p_empty + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_done + 1);
-  static_assert(1 + 2 * AT_KST + 2 * AT_VST + 2 * AT_NS + 4 + 1 + 1 <= 32, "barrier block is 256 bytes");
-  constexpr bool SPLIT = (SW == 8);
-  static_assert(!PT || (BN == 64 && SW == 4 && !CW3), "P~ in tensor memory is built for the default configuration");
-  // timing ablations (RVB_ATTN_POLY = 8 | 9 | 10 | 11, WRONG RESULTS by construction; tools/attn_bench.py): which part of
-  // the softmax warps' tile loop costs what
-  constexpr bool ABL_NOEXP = (POLY == 8 || POLY == 11);   // no MUFU.EX2: P~ = x - m
-  constexpr bool ABL_NOSTS = (POLY == 9 || POLY == 11);   // P~ is not written to shared memory
-  constexpr bool ABL_NOMAX = (POLY == 10 || POLY == 11);  // no scale / key bias / tile maximum
-  constexpr bool ABL_NOPV = (POLY == 12);                 // the control thread skips the PV products (barriers kept)
-  constexpr bool ABL_NOQK = (POLY == 13);                 // the control thread skips the QK products (barriers kept)
-  constexpr bool ABL_NOFENCE = (POLY == 14);              // no fence.proxy.async after the P~ stores
-  constexpr bool ABL_NOLD = (POLY == 15);                 // no tcgen05.ld of S (softmax on stale registers)
-  constexpr bool ABL_NOTMAWAIT = (POLY == 16);            // the MMAs do not wait for the K'' / V tiles to land
-  constexpr bool ABL_NOMMA = (POLY == 17);                // neither product is issued
-  constexpr int CW = BN * 4 / SW;   // S columns per thread and tile
-  constexpr int OW = AT_DK * 4 / SW;  // O columns per thread (rescale, epilogue)
-  static_assert(SW == 4 || (SW == 8 && BN == 64), "8 softmax warps are built for 64-key tiles");
-  float* s_xch = reinterpret_cast<float*>(bars + 32);   // SPLIT: [2 tile parity][2 halves][128 rows] partial tile maxima
-  float* s_sumx = s_xch + 512;                          // SPLIT: [2 halves][128 rows] partial row sums
-  float* s_bias = SPLIT ? s_sumx + 256 : s_xch;         // [ntiles * BN]: key bias * scale*log2e, -inf when masked
+  uint8_t* sK = sQ + AT_Q_BYTES;               // AT_ST stages
+  uint8_t* sV = sK + AT_ST * AT_TILE_BYTES;    // AT_ST stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + AT_ST * AT_TILE_BYTES);
+  uint64_t* q_full = bars;
+  uint64_t* k_full = bars + 1;             // [AT_ST]
+  uint64_t* k_empty = k_full + AT_ST;      // [AT_ST]
+  uint64_t* v_full = k_empty + AT_ST;      // [AT_ST]
+  uint64_t* v_empty = v_full + AT_ST;      // [AT_ST]
+  static_assert(1 + 4 * AT_ST <= 32, "barrier block is 256 bytes");
+  float* s_bias = reinterpret_cast<float*>(bars + 32);   // [ntiles * AT_BN]: key bias * scale*log2e, -inf when masked
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qtile = blockIdx.x, h = blockIdx.y, g = blockIdx.z;
@@ -177,841 +80,188 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   auto vis_hi = [&](int i) { return p.chunk > 0 ? min(klen, (i / p.chunk + 1) * p.chunk) : klen; };
   const int jt0 = vis_lo(q0) / AT_BN;
   const int ntiles = max(0, (vis_hi(q0 + AT_BM - 1) + AT_BN - 1) / AT_BN - jt0);
-
-  const long long qrow = (long long)g * p.Tq + q0;
   const long long krow0 = (long long)g * p.Tk;
-  // TMA loads of K'' / V tile n into their rings (control thread only; the wait on the ring slot passes at first use)
-  auto load_k = [&](int n) {
-    const int st = n % AT_KST, use = n / AT_KST;
-    mbar_wait(&k_empty[st], (use & 1) ^ 1);
-    mbar_expect_tx(&k_full[st], AT_TILE_BYTES);
-    tma_load_2d(sK + st * AT_TILE_BYTES, &tmK, &k_full[st], h * AT_DK, (int)(krow0 + (jt0 + n) * AT_BN));
-  };
-  auto load_v = [&](int j) {
-    const int st = j % AT_VST;
-    mbar_wait(&v_empty[st], ((j / AT_VST) & 1) ^ 1);
-    mbar_expect_tx(&v_full[st], AT_TILE_BYTES);
-    tma_load_2d(sV + st * AT_TILE_BYTES, &tmV, &v_full[st], h * AT_DK, (int)(krow0 + (jt0 + j) * AT_BN));
-  };
-  if (warp == SW) {
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      for (int i = 0; i < AT_KST; ++i) {
-        mbar_init(&k_full[i], 1);
-        mbar_init(&k_empty[i], 1);
-      }
-      for (int i = 0; i < AT_NS; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&s_empty[i], PT ? 1 : SW);   // PT: released by PV(j)'s commit, otherwise by the softmax warps' pull
-      }
-      for (int i = 0; i < AT_VST; ++i) {
-        mbar_init(&v_full[i], 1);
-        mbar_init(&v_empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&p_full[i], SW);
-        mbar_init(&p_empty[i], (PT && i == 0) ? SW : 1);   // PT: p_full[0..2] = one "P~ written" barrier per S buffer
-      }
-      mbar_init(o_done, 1);
-      fence_barrier_init();
-      tma_prefetch_desc(&tmQ);
-      tma_prefetch_desc(&tmK);
-      tma_prefetch_desc(&tmV);
-      // The first loads go out BEFORE the CTA-wide barrier: their latency overlaps the key-bias fill and the TMEM
-      // allocation instead of following them (the per-CTA fixed cost was 22 % of the kernel, tools/attn_bench.py --sweep).
-      if (!CW3 && ntiles > 0) {
-        mbar_expect_tx(q_full, AT_Q_BYTES);
-        tma_load_2d(sQ, &tmQ, q_full, h * AT_DK, (int)qrow);
-        for (int n = 0; n < AT_KST && n < ntiles; ++n) load_k(n);
-        for (int n = 0; n < AT_VST - 1 && n < ntiles; ++n) load_v(n);
-      }
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < AT_ST; ++i) {
+      mbar_init(&k_full[i], 1);
+      mbar_init(&k_empty[i], 8);   // lane 0 of every consumer warp
+      mbar_init(&v_full[i], 1);
+      mbar_init(&v_empty[i], 8);
     }
-    __syncwarp();
-    tmem_alloc(tmem_ptr, AT_TMEM_COLS);
-    tmem_relinquish();
-  } else if (warp < SW) {
+    fence_barrier_init();
+  }
+  {
     // key bias row of this (group, head), pre-scaled; masked keys -> -inf
     const float* kb = p.key_bias ? p.key_bias + ((long long)g * p.H + h) * p.Tk : nullptr;
-    for (int kk = threadIdx.x; kk < ntiles * AT_BN; kk += 32 * SW) {
+    for (int kk = threadIdx.x; kk < ntiles * AT_BN; kk += AT_THREADS) {
       const int key = jt0 * AT_BN + kk;
       s_bias[kk] = (key < klen) ? (kb ? __ldg(kb + key) * p.scale_log2 : 0.f) : -INFINITY;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t tmem_o = tmem_base + 2 * AT_BN;
-  auto s_col = [&](int sb) -> uint32_t { return tmem_base + (sb < 2 ? sb * AT_BN : 2 * AT_BN + 64); };
 
-  if (warp >= SW) {
-    if constexpr (CW3 && BN == 64) asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-    if (lane == 0 && ntiles > 0 && (!CW3 || warp < SW + 3)) {
-      // ------------------------------------------------------------ TMA + MMA control thread(s)
-      // instruction descriptors: D=f32, A=B=bf16.  QK: N=128, both K-major.  PV: N=64, B (V) MN-major (bit 16).
-      constexpr uint32_t idesc_qk =
-          (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AT_BN >> 3) << 17) | ((128u >> 4) << 24);
-      constexpr uint32_t idesc_pv =
-          (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
-      const int total = ntiles;
-      auto issue_qk = [&](int n) {
-        const int st = n % AT_KST, sb = n % AT_NS;
-        if (!ABL_NOTMAWAIT) mbar_wait(&k_full[st], (n / AT_KST) & 1);
-        mbar_wait(&s_empty[sb], ((n / AT_NS) & 1) ^ 1);
-        tc_fence_after();
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(sQ));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(sK + st * AT_TILE_BYTES));
-#pragma unroll
-        for (int k = 0; k < ((ABL_NOQK || ABL_NOMMA) ? 0 : AT_DK / 16); ++k)
-          umma_f16(s_col(sb), adesc + 2 * k, bdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[sb]);
-        umma_commit(&k_empty[st]);
-      };
-      auto issue_pv = [&](int j) {
-        const int pb = PT ? j % AT_NS : (j & 1);  // O += P~(j) . V(j)
-        const int vs = j % AT_VST;
-        if (!ABL_NOTMAWAIT) mbar_wait(&v_full[vs], (j / AT_VST) & 1);
-        mbar_wait(&p_full[pb], PT ? (j / AT_NS) & 1 : (j >> 1) & 1);
-        tc_fence_after();
-        const uint64_t vdesc = make_sw128_kmajor_desc(smem_u32(sV + vs * AT_TILE_BYTES));  // MN-major view
-        if constexpr (PT) {
-#pragma unroll
-          for (int ks = 0; ks < ((ABL_NOPV || ABL_NOMMA) ? 0 : AT_BN / 16); ++ks) {
-            // A: 16 keys = 8 packed columns of the S buffer this tile's P~ overwrote; B: 16 key rows of 128 B
-            const uint64_t bd = vdesc + (uint64_t)(ks * ((16 * 128) >> 4));
-            umma_f16_ts(tmem_o, s_col(pb) + 8 * ks, bd, idesc_pv, (j | ks) != 0);
-          }
-          umma_commit(&s_empty[pb]);
-        } else {
-          const uint64_t pdesc = make_sw128_kmajor_desc(smem_u32(sP + pb * AT_P_BYTES));
-#pragma unroll
-          for (int ks = 0; ks < ((ABL_NOPV || ABL_NOMMA) ? 0 : AT_BN / 16); ++ks) {
-            // A: 16 keys = 32 B inside the 64-key K-block (ks / 4); B: 16 key rows of 128 B
-            const uint64_t a = pdesc + (uint64_t)((ks >> 2) * (AT_Q_BYTES >> 4) + (ks & 3) * 2);
-            const uint64_t bd = vdesc + (uint64_t)(ks * ((16 * 128) >> 4));
-            umma_f16(tmem_o, a, bd, idesc_pv, (j | ks) != 0);
-          }
-          umma_commit(&p_empty[pb]);
-        }
-        umma_commit(&v_empty[vs]);
-        if (j + 1 == ntiles) umma_commit(o_done);
-      };
-      if constexpr (!CW3) {
-        // Q, K''(0 .. AT_KST-1), V(0 .. AT_VST-2) were requested in the prologue
-        mbar_wait(q_full, 0);
-        for (int n = 0; n < AT_NS && n < total; ++n) issue_qk(n);
-        for (int i = 0; i < total; ++i) {
-          // Keep the QK products AT_NS tiles ahead: S buffer (i % AT_NS) is free as soon as the softmax warps have pulled
-          // S(i) out of TMEM (they signal that BEFORE doing the exponentials), so QK(i+AT_NS) is queued long before it
-          // is needed.  K'' tiles are requested two tiles before their product.
-          if constexpr (PT) {
-            // the S buffer of tile i comes back when PV(i) retires: QK(i + AT_NS - 1) waits for PV(i - 1), issued a whole
-            // iteration ago, so the products still run AT_NS - 1 tiles ahead of the softmax warps
-            issue_pv(i);
-            if (i >= 1 && i - 1 + AT_NS < total) issue_qk(i - 1 + AT_NS);
-            if (i + AT_KST < total) load_k(i + AT_KST);
-          } else {
-            if (i + AT_NS < total) issue_qk(i + AT_NS);
-            if (i + AT_KST < total) load_k(i + AT_KST);  // stage of K''(i): released by QK(i)'s commit, long done
-            issue_pv(i);
-          }
-          // V(i + AT_VST - 1) goes into the stage PV(i-1) read; that product was issued a whole iteration ago
-          if (i + AT_VST - 1 < ntiles) load_v(i + AT_VST - 1);
-        }
-      } else if (warp == SW) {
-        // ---- loader: runs ahead as far as the K'' (AT_KST) and V (AT_VST) rings allow
-        mbar_expect_tx(q_full, AT_Q_BYTES);
-        tma_load_2d(sQ, &tmQ, q_full, h * AT_DK, (int)qrow);
-        for (int n = 0; n < total; ++n) {
-          load_k(n);
-          load_v(n);
-        }
-      } else if (warp == SW + 1) {
-        // ---- QK issuer: S(n) as soon as K''(n) has landed and the softmax warps have pulled S(n - AT_NS)
-        mbar_wait(q_full, 0);
-        for (int n = 0; n < total; ++n) issue_qk(n);
-      } else {
-        // ---- PV issuer: O += P~(j) V(j) as soon as the softmax warps have published P~(j)
-        for (int j = 0; j < total; ++j) issue_pv(j);
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- softmax warps: thread = query row (x column half)
-    if constexpr (CW3 && BN == 64) asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-    const int wq = warp & 3, hh = warp >> 2;   // TMEM lane quarter; column half (always 0 when SW == 4)
-    const int r = wq * 32 + lane;
-    const bool pipe = (p.pipe != 0) && (CW == 64) && !PT;
-    const uint32_t lane_addr = ((uint32_t)(wq * 32) << 16);
-    const int c0 = hh * CW, ob = hh * OW;
-    auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + wq) : "memory"); };
-    float m_run = -INFINITY, row_sum = 0.f;  // m_run stays -inf until the row has seen a visible key
-    // The thread's part of an S row is pulled out of TMEM with back-to-back loads and ONE wait.  (A variant that
-    // prefetched tile j+1 into a second register copy before the arithmetic of tile j needed ~230 registers, spilled at
-    // the 168 available with 2 CTAs / SM and measured 0.62 ms instead of 0.43 ms per encoder layer: removed.)
-    auto pull = [&](int j, uint32_t(&dst)[CW]) {
-      const int sb = j % AT_NS;
-      mbar_wait(&s_full[sb], (j / AT_NS) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < (ABL_NOLD ? 0 : CW); c += 32) tmem_ld_32x32(s_col(sb) + lane_addr + c0 + c, dst + c);
-    };
-    // PIPE (CW == 64 only): S(j+1) is pulled in two halves INSIDE tile j's exponential loop, each half into the registers
-    // the loop has just finished with — the tcgen05.ld latency hides behind the other half's exponentials without a
-    // second register copy of the tile (the full-copy prefetch variant spilled).
-    auto pull_half = [&](int j, int half, uint32_t(&dst)[CW]) {
-      const int sb = j % AT_NS;
-      if (half == 0) {
-        mbar_wait(&s_full[sb], (j / AT_NS) & 1);
-        tc_fence_after();
-      }
-      if (!ABL_NOLD) tmem_ld_32x32(s_col(sb) + lane_addr + c0 + 32 * half, dst + 32 * half);
-    };
-    auto tile = [&](int j, uint32_t(&sv)[CW]) {
-      const int sb = j % AT_NS, pb = j & 1;
-      if (!pipe || j == 0) pull(j, sv);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (!PT && lane == 0) mbar_arrive(&s_empty[sb]);   // the S buffer goes back to the MMA issuer as early as possible
-      const uint32_t bias_addr = smem_u32(s_bias + j * AT_BN + c0);
-      // x = s * scale*log2e + key bias (masked keys: -inf), kept in place of the raw scores; tile maximum
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // 4 independent chains
-      const float2 sc2 = make_float2(p.scale_log2, p.scale_log2);
-#pragma unroll
-      for (int e = 0; e < (ABL_NOMAX ? 0 : CW); e += 4) {
-        const float4 b4 = lds128(bias_addr + e * 4);
-        // packed FFMA2: two scores per instruction
-        const float2 x01 = ffma2(make_float2(__uint_as_float(sv[e + 0]), __uint_as_float(sv[e + 1])), sc2,
-                                 make_float2(b4.x, b4.y));
-        const float2 x23 = ffma2(make_float2(__uint_as_float(sv[e + 2]), __uint_as_float(sv[e + 3])), sc2,
-                                 make_float2(b4.z, b4.w));
-        sv[e + 0] = __float_as_uint(x01.x);
-        sv[e + 1] = __float_as_uint(x01.y);
-        sv[e + 2] = __float_as_uint(x23.x);
-        sv[e + 3] = __float_as_uint(x23.y);
-        mx[(e >> 2) & 3] = fmax3(mx[(e >> 2) & 3], x01.x, x01.y);
-        mx[((e >> 2) + 2) & 3] = fmax3(mx[((e >> 2) + 2) & 3], x23.x, x23.y);
-      }
-      float tmax = ABL_NOMAX ? 0.f : fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      if (p.chunk > 0) {
-        // boundary tiles of the chunk mask (warp-uniform test over the warp's 32 rows; visibility bounds are
-        // non-decreasing in the row index): hide the keys outside [lo, hi) of this row and redo the tile maximum
-        const int kbase = (jt0 + j) * AT_BN + c0;           // key index of this thread's column 0
-        const int i0 = q0 + wq * 32;
-        if (kbase < vis_lo(i0 + 31) || kbase + CW > vis_hi(i0)) {
-          const int lo = vis_lo(q0 + r) - kbase, hi = vis_hi(q0 + r) - kbase;  // visible columns: lo <= e < hi
-          tmax = -INFINITY;
-#pragma unroll
-          for (int e = 0; e < CW; ++e) {
-            const float x = (e >= lo && e < hi) ? __uint_as_float(sv[e]) : -INFINITY;
-            sv[e] = __float_as_uint(x);
-            tmax = fmaxf(tmax, x);
-          }
-        }
-      }
-      if (p.key_bits) {
-        // arbitrary visibility (prefix-tree self-attention: a node sees its ancestors): one bit per key of this row
-        const int kbase = (jt0 + j) * AT_BN + c0;
-        const uint32_t* mw = p.key_bits + ((long long)g * p.Tq + min(q0 + r, p.Tq - 1)) * p.bits_ld + (kbase >> 5);
-        tmax = -INFINITY;
-#pragma unroll
-        for (int wi = 0; wi < CW / 32; ++wi) {
-          const uint32_t word = __ldg(mw + wi);
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            const float x = ((word >> e) & 1u) ? __uint_as_float(sv[wi * 32 + e]) : -INFINITY;
-            sv[wi * 32 + e] = __float_as_uint(x);
-            tmax = fmaxf(tmax, x);
-          }
-        }
-      }
-      if (SPLIT) {  // the row's tile maximum = max of the two halves (both halves must move m_run identically)
-        s_xch[(j & 1) * 256 + hh * 128 + r] = tmax;
-        pair_sync();
-        tmax = fmaxf(tmax, s_xch[(j & 1) * 256 + (hh ^ 1) * 128 + r]);
-      }
-      if (j == 0) {
-        m_run = tmax;  // PV(0) overwrites O: nothing to rescale
-      } else {
-        const bool raise = tmax > m_run + 8.f;
-        if (__any_sync(0xffffffffu, raise)) {
-          // Lazy rescale (rare): O and the row sum move to the new maximum.  The last product issued, PV(j-1), must
-          // have retired before O is touched; PV(j) is not issued before every softmax warp arrives on p_full(j).
-          if constexpr (PT) mbar_wait(&s_empty[(j - 1) % AT_NS], ((j - 1) / AT_NS) & 1);
-          else mbar_wait(&p_empty[(j - 1) & 1], ((j - 1) >> 1) & 1);
-          tc_fence_after();
-          const float m_new = raise ? tmax : m_run;
-          // 1 for the rows that keep their maximum; 0 for rows that see their first visible key only now (their O
-          // row and row sum are zero so far) — never exp2(-inf - -inf)
-          const float f = (m_new == -INFINITY) ? 1.f : fast_exp2(m_run - m_new);
-          m_run = m_new;
-          row_sum *= f;
-#pragma unroll 1
-          for (int c = ob; c < ob + OW; c += 32) {
-            uint32_t ov[32];
-            tmem_ld_32x32(tmem_o + lane_addr + c, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) ov[e] = __float_as_uint(__uint_as_float(ov[e]) * f);
-            tmem_st_32x32(tmem_o + lane_addr + c, ov);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-        }
-      }
-      float2 sm01 = make_float2(0.f, 0.f), sm23 = make_float2(0.f, 0.f);
-      const float m_eff = (m_run == -INFINITY) ? 0.f : m_run;  // no visible key yet: every x is -inf -> p = 0
-      const float2 one2 = make_float2(1.f, 1.f), negm2 = make_float2(-m_eff, -m_eff);
-      // the polynomial exp2 path needs finite arguments: tiles fully inside [0, klen) without a chunk-mask boundary
-      const bool poly_ok = (POLY < 8) && (p.chunk == 0) && (p.key_bits == nullptr) && ((jt0 + j + 1) * AT_BN <= klen) && (m_run != -INFINITY) &&
-                           __all_sync(0xffffffffu, m_run != -INFINITY);
-      // P~ goes to shared memory chunk by chunk (8 keys = 16 bytes) as it is produced, so only one chunk of packed
-      // probabilities is ever live in registers.  The buffer was last read by PV(j-2), which has had a whole tile of
-      // exponentials to retire: this wait is practically free.
-      if (!PT) mbar_wait(&p_empty[pb], ((j >> 1) & 1) ^ 1);
-#pragma unroll
-      for (int e = 0; e < CW; e += 8) {
-        uint32_t w[4];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          // x - m and the running sums as packed FFMA2 (x * 1 + (-m), p * 1 + sum: exact)
-          const int f = e + 4 * q;
-          const float2 d01 = ffma2(make_float2(__uint_as_float(sv[f + 0]), __uint_as_float(sv[f + 1])), one2, negm2);
-          const float2 d23 = ffma2(make_float2(__uint_as_float(sv[f + 2]), __uint_as_float(sv[f + 3])), one2, negm2);
-          float2 p01 = ABL_NOEXP ? d01 : make_float2(fast_exp2(d01.x), fast_exp2(d01.y));
-          // POLY > 0: in every POLY-th group of four (POLY = 1: half, 2: a quarter of all exponentials) the second pair on the FMA pipe instead of MUFU (only when every key
-          // of the tile is visible: masked keys carry -inf, which the polynomial path does not produce exact zeros for)
-          float2 p23;
-          if (ABL_NOEXP) p23 = d23;
-          else if ((POLY == 1 || POLY == 2) && poly_ok && ((f >> 2) % (POLY > 0 ? POLY : 1)) == 0) p23 = exp2_poly2(d23);
-          else p23 = make_float2(fast_exp2(d23.x), fast_exp2(d23.y));
-          if (AT_TRUNC_P && POLY != 3) {   // POLY == 3: A/B variant with F2FP rounding and an unrounded row sum
-            // P~ = the exponentials TRUNCATED to bf16 (upper 16 bits: one ALU byte-permute per pair) instead of rounded
-            // by F2FP — the conversion shares the XU pipe with MUFU.EX2, the pipe that bounds this kernel (ncu: xu 54 %,
-            // everything else < 20 %).  The row sum adds the same truncated values, so O / row_sum is normalised by
-            // exactly the weights the PV product used.
-            const uint32_t b0 = __float_as_uint(p01.x) & 0xffff0000u, b1 = __float_as_uint(p01.y) & 0xffff0000u;
-            const uint32_t b2 = __float_as_uint(p23.x) & 0xffff0000u, b3 = __float_as_uint(p23.y) & 0xffff0000u;
-            w[2 * q + 0] = __byte_perm(b0, b1, 0x7632);
-            w[2 * q + 1] = __byte_perm(b2, b3, 0x7632);
-            p01 = make_float2(__uint_as_float(b0), __uint_as_float(b1));
-            p23 = make_float2(__uint_as_float(b2), __uint_as_float(b3));
-          } else {
-            w[2 * q + 0] = pack_bf16x2(p01.x, p01.y);
-            w[2 * q + 1] = pack_bf16x2(p23.x, p23.y);
-          }
-          sm01 = ffma2(p01, one2, sm01);
-          sm23 = ffma2(p23, one2, sm23);
-        }
-        // 8 keys = one 16-byte chunk of this row inside K-block (key / 64); SWIZZLE_128B: chunk ^= row % 8
-        const int kc = c0 + e;
-        uint8_t* blk = sP + pb * AT_P_BYTES + (kc >> 6) * AT_Q_BYTES + r * 128;
-        const int ch = ((kc & 63) >> 3) ^ (r & 7);
-        if constexpr (PT) {   // packed P~ replaces the consumed scores in place: word i = keys (2i, 2i+1)
-          sv[(e >> 1) + 0] = w[0];
-          sv[(e >> 1) + 1] = w[1];
-          sv[(e >> 1) + 2] = w[2];
-          sv[(e >> 1) + 3] = w[3];
-        } else if (!ABL_NOSTS) *reinterpret_cast<uint4*>(blk + ch * 16) = make_uint4(w[0], w[1], w[2], w[3]);
-        else if (w[0] == 0x12345678u && w[1] == w[2] + w[3]) *reinterpret_cast<uint4*>(blk) = make_uint4(w[0], w[1], w[2], w[3]);
-        if constexpr (CW == 64) {
-          if (pipe && j + 1 < ntiles) {
-            if (e == 24) pull_half(j + 1, 0, sv);   // columns [0, 32) of this tile are consumed
-            if (e == 56) pull_half(j + 1, 1, sv);
-          }
-        }
-      }
-      const float sm[4] = {sm01.x, sm01.y, sm23.x, sm23.y};
-      row_sum += (sm[0] + sm[1]) + (sm[2] + sm[3]);
-      if constexpr (PT) {
-        if constexpr (CW == 64) tmem_st_32x32(s_col(sb) + lane_addr, sv);   // P~ row over the first 32 columns of its S row
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[sb]);
-      } else {
-        if (!ABL_NOFENCE) fence_proxy_async();  // generic-proxy writes of P~ -> visible to the tensor-core (async) proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[pb]);
-      }
-    };
-    {
-      uint32_t sv[CW];
-#pragma unroll 1
-      for (int j = 0; j < ntiles; ++j) tile(j, sv);
-    }
-    // ---- epilogue: O / row_sum -> bf16 -> global
-    if (SPLIT) {
-      s_sumx[hh * 128 + r] = row_sum;
-      pair_sync();
-      row_sum += s_sumx[(hh ^ 1) * 128 + r];
-    }
-    const int row = q0 + r;
-    if (ntiles > 0) {
-      mbar_wait(o_done, 0);
-      tc_fence_after();
-    }
-    const float inv = row_sum > 0.f ? 1.f / row_sum : 0.f;
-    bf16* orow = p.out + ((long long)g * p.Tq + row) * p.ldo + h * AT_DK;
-#pragma unroll 1
-    for (int c = ob; c < ob + OW; c += 32) {
-      uint32_t ov[32];
-      if (ntiles > 0) {
-        tmem_ld_32x32(tmem_o + lane_addr + c, ov);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int e = 0; e < 32; ++e) ov[e] = 0u;
-      }
-      if (row < p.Tq) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(ov[8 * q + 0]) * inv, __uint_as_float(ov[8 * q + 1]) * inv);
-          u.y = pack_bf16x2(__uint_as_float(ov[8 * q + 2]) * inv, __uint_as_float(ov[8 * q + 3]) * inv);
-          u.z = pack_bf16x2(__uint_as_float(ov[8 * q + 4]) * inv, __uint_as_float(ov[8 * q + 5]) * inv);
-          u.w = pack_bf16x2(__uint_as_float(ov[8 * q + 6]) * inv, __uint_as_float(ov[8 * q + 7]) * inv);
-          reinterpret_cast<uint4*>(orow + c)[q] = u;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == SW) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, AT_TMEM_COLS);
-  }
-}
-
-// =====================================================================================================================
-// PERSISTENT variant (RVB_ATTN_PERSIST=1; measured slower, see launch_attention_tc): one CTA per SM slot (2 x #SMs CTAs) loops over
-// (query tile, head, group) items.  tools/attn_bench.py --sweep showed 22 % of the one-item-per-CTA kernel's time was
-// per-CTA fixed cost (launch, barrier init, TMEM allocation, first TMA round trip, key-bias fill, pipeline fill, drain).
-// Here TMEM and the barriers are set up once and ALL rings (K'', V, S / P~) keep running across item boundaries: four
-// cursors — K'' load, V load, QK issue, PV issue — walk the same (item, tile) sequence at different leads, so the next
-// item's Q and first tiles are in flight while the softmax warps finish the current one; the key-bias row of the next
-// item is fetched into registers an item ahead.  P~ lives in tensor memory (see PT above).  Same arithmetic, same
-// results as attention_tc_kernel<64, 4, 0, false, true>.
-struct AtItem {
-  int g, h, q0, klen, jt0, ntiles;
-};
-
-__device__ __forceinline__ AtItem at_item(const AttnTcParams& p, int it, int nq) {
-  AtItem a;
-  const int qt = it % nq;
-  a.h = (it / nq) % p.H;
-  a.g = it / (nq * p.H);
-  a.q0 = qt * AT_BM;
-  a.klen = p.Tk;
-  if (p.k_lens) a.klen = min(a.klen, __ldg(p.k_lens + a.g));
-  const int lo = (p.chunk > 0 && p.left >= 0) ? max(0, (a.q0 / p.chunk - p.left) * p.chunk) : 0;
-  const int last = a.q0 + AT_BM - 1;
-  const int hi = p.chunk > 0 ? min(a.klen, (last / p.chunk + 1) * p.chunk) : a.klen;
-  a.jt0 = lo / 64;
-  a.ntiles = max(0, (hi + 63) / 64 - a.jt0);
-  return a;
-}
-
-// walks the tiles of the CTA's items in order; `n` counts tiles globally (ring slots and barrier phases follow it)
-struct AtCursor {
-  int k;        // index into this CTA's item list
-  int j;        // tile inside the item
-  int n;        // global tile count
-  int ne;       // number of non-empty items before the current one
-  AtItem it;
-  bool valid;
-};
-
-__device__ __forceinline__ void at_cursor_seek(const AttnTcParams& p, AtCursor& c, int n_items, int nq) {
-  // position on the first item at or after c.k that has tiles
-  for (;;) {
-    const long long id = (long long)blockIdx.x + (long long)c.k * gridDim.x;
-    if (id >= n_items) {
-      c.valid = false;
-      return;
-    }
-    c.it = at_item(p, (int)id, nq);
-    if (c.it.ntiles > 0) {
-      c.valid = true;
-      return;
-    }
-    ++c.k;
-  }
-}
-__device__ __forceinline__ void at_cursor_init(const AttnTcParams& p, AtCursor& c, int n_items, int nq) {
-  c.k = 0;
-  c.j = 0;
-  c.n = 0;
-  c.ne = 0;
-  at_cursor_seek(p, c, n_items, nq);
-}
-__device__ __forceinline__ void at_cursor_next(const AttnTcParams& p, AtCursor& c, int n_items, int nq) {
-  ++c.n;
-  if (++c.j == c.it.ntiles) {
-    c.j = 0;
-    ++c.k;
-    ++c.ne;
-    at_cursor_seek(p, c, n_items, nq);
-  }
-}
-
-constexpr int ATP_KST = 5, ATP_VST = 4, ATP_NS = 3;
-constexpr bool ATP_TRUNC = false;   // true: P~ truncated on the ALU (see AT_TRUNC_P)
-constexpr uint32_t ATP_TILE = 64 * AT_DK * 2;   // 8 KB
-constexpr uint32_t ATP_SMEM_FIXED = 2 * AT_Q_BYTES + (ATP_KST + ATP_VST) * ATP_TILE + 1024 + 384;
-
-__global__ void __launch_bounds__(160, 2)
-attention_tcp_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const AttnTcParams p, int n_items, int nq, int bias_len) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                               // 2 buffers
-  uint8_t* sK = sQ + 2 * AT_Q_BYTES;
-  uint8_t* sV = sK + ATP_KST * ATP_TILE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ATP_VST * ATP_TILE);
-  uint64_t* q_full = bars;                          // [2]
-  uint64_t* q_empty = q_full + 2;                   // [2]
-  uint64_t* k_full = q_empty + 2;                   // [KST]
-  uint64_t* k_empty = k_full + ATP_KST;
-  uint64_t* v_full = k_empty + ATP_KST;             // [VST]
-  uint64_t* v_empty = v_full + ATP_VST;
-  uint64_t* s_full = v_empty + ATP_VST;             // [NS]
-  uint64_t* s_empty = s_full + ATP_NS;              // [NS]  (PV(n) retired: S / P~ buffer free)
-  uint64_t* p_full = s_empty + ATP_NS;              // [NS]  (P~(n) written)
-  uint64_t* o_done = p_full + ATP_NS;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_done + 1);
-  static_assert(4 + 2 * ATP_KST + 2 * ATP_VST + 3 * ATP_NS + 1 + 1 <= 48, "barrier block is 384 bytes");
-  float* s_bias = reinterpret_cast<float*>(bars + 48);   // [2][bias_len]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 4) {
-    if (lane == 0) {
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&q_full[i], 1);
-        mbar_init(&q_empty[i], 1);
-      }
-      for (int i = 0; i < ATP_KST; ++i) {
-        mbar_init(&k_full[i], 1);
-        mbar_init(&k_empty[i], 1);
-      }
-      for (int i = 0; i < ATP_VST; ++i) {
-        mbar_init(&v_full[i], 1);
-        mbar_init(&v_empty[i], 1);
-      }
-      for (int i = 0; i < ATP_NS; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&s_empty[i], 1);
-        mbar_init(&p_full[i], 4);
-      }
-      mbar_init(o_done, 1);
-      fence_barrier_init();
+  if (warp == 8) {
+    // ---------------------------------------------------------------- TMA producer
+    if (lane == 0 && ntiles > 0) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
       tma_prefetch_desc(&tmV);
+      mbar_expect_tx(q_full, AT_Q_BYTES);
+      tma_load_2d(sQ, &tmQ, q_full, h * AT_DK, (int)((long long)g * p.Tq + q0));
+      for (int n = 0; n < ntiles; ++n) {
+        const int st = n % AT_ST, ph = ((n / AT_ST) & 1) ^ 1;
+        const int krow = (int)(krow0 + (jt0 + n) * AT_BN);
+        mbar_wait(&k_empty[st], ph);
+        mbar_expect_tx(&k_full[st], AT_TILE_BYTES);
+        tma_load_2d(sK + st * AT_TILE_BYTES, &tmK, &k_full[st], h * AT_DK, krow);
+        mbar_wait(&v_empty[st], ph);
+        mbar_expect_tx(&v_full[st], AT_TILE_BYTES);
+        tma_load_2d(sV + st * AT_TILE_BYTES, &tmV, &v_full[st], h * AT_DK, krow);
+      }
     }
-    __syncwarp();
-    tmem_alloc(tmem_ptr, 256);
-    tmem_relinquish();
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t tmem_o = tmem_base + 128;
-  auto s_col = [&](int sb) -> uint32_t { return tmem_base + (sb < 2 ? sb * 64 : 192); };
 
-  if (warp == 4) {
-    if (lane == 0) {
-      // ---------------------------------------------------------------- control thread: four cursors over one sequence
-      constexpr uint32_t idesc_qk = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(64 >> 3) << 17) | ((128u >> 4) << 24);
-      constexpr uint32_t idesc_pv =
-          (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
-      AtCursor ck, cv, cq, cp;
-      at_cursor_init(p, ck, n_items, nq);
-      cv = ck;
-      cq = ck;
-      cp = ck;
-      // K''(n) (and, at an item's first tile, its Q) — false when the Q buffer is still being read by the item two
-      // back: the caller retries later.  Never blocks on the Q ring: with one-tile items the K'' cursor would otherwise
-      // wait for a QK product that this same thread has not issued yet.
-      auto try_load_k = [&]() -> bool {
-        if (ck.j == 0) {
-          const int qb = ck.ne & 1;
-          if (!mbar_try_wait(&q_empty[qb], ((ck.ne >> 1) & 1) ^ 1)) return false;
-          mbar_expect_tx(&q_full[qb], AT_Q_BYTES);
-          tma_load_2d(sQ + qb * AT_Q_BYTES, &tmQ, &q_full[qb], ck.it.h * AT_DK,
-                      (int)((long long)ck.it.g * p.Tq + ck.it.q0));
-        }
-        const int st = ck.n % ATP_KST;
-        mbar_wait(&k_empty[st], ((ck.n / ATP_KST) & 1) ^ 1);   // QK(n - KST) was issued (callers keep n - cq.n < KST)
-        mbar_expect_tx(&k_full[st], ATP_TILE);
-        tma_load_2d(sK + st * ATP_TILE, &tmK, &k_full[st], ck.it.h * AT_DK,
-                    (int)((long long)ck.it.g * p.Tk + (ck.it.jt0 + ck.j) * 64));
-        at_cursor_next(p, ck, n_items, nq);
-        return true;
-      };
-      auto load_v = [&]() {
-        const int st = cv.n % ATP_VST;
-        mbar_wait(&v_empty[st], ((cv.n / ATP_VST) & 1) ^ 1);
-        mbar_expect_tx(&v_full[st], ATP_TILE);
-        tma_load_2d(sV + st * ATP_TILE, &tmV, &v_full[st], cv.it.h * AT_DK,
-                    (int)((long long)cv.it.g * p.Tk + (cv.it.jt0 + cv.j) * 64));
-        at_cursor_next(p, cv, n_items, nq);
-      };
-      auto issue_qk = [&]() {
-        const int st = cq.n % ATP_KST, sb = cq.n % ATP_NS, qb = cq.ne & 1;
-        if (cq.j == 0) mbar_wait(&q_full[qb], (cq.ne >> 1) & 1);
-        mbar_wait(&k_full[st], (cq.n / ATP_KST) & 1);
-        mbar_wait(&s_empty[sb], ((cq.n / ATP_NS) & 1) ^ 1);
-        tc_fence_after();
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(sQ + qb * AT_Q_BYTES));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(sK + st * ATP_TILE));
+  // ------------------------------------------------------------------ consumer warpgroups
+  const int wg = warp >> 2, wl = warp & 3;
+  // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16) and its key / dk columns
+  // 8j + 2(l%4) + {0, 1}, j = 0..7
+  const int rloc = wg * 64 + wl * 16 + (lane >> 2);
+  const int row[2] = {q0 + rloc, q0 + rloc + 8};
+  const int cq = 2 * (lane & 3);
+  float o[32];
 #pragma unroll
-        for (int k = 0; k < AT_DK / 16; ++k) umma_f16(s_col(sb), adesc + 2 * k, bdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[sb]);
-        umma_commit(&k_empty[st]);
-        if (cq.j + 1 == cq.it.ntiles) umma_commit(&q_empty[qb]);   // the item's last read of its Q buffer
-        at_cursor_next(p, cq, n_items, nq);
-      };
-      auto issue_pv = [&]() {
-        const int sb = cp.n % ATP_NS, vs = cp.n % ATP_VST;
-        mbar_wait(&v_full[vs], (cp.n / ATP_VST) & 1);
-        mbar_wait(&p_full[sb], (cp.n / ATP_NS) & 1);
-        tc_fence_after();
-        const uint64_t vdesc = make_sw128_kmajor_desc(smem_u32(sV + vs * ATP_TILE));   // MN-major view
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, row_sum[2] = {0.f, 0.f};   // row_sum: this thread's columns only
+  if (ntiles > 0) mbar_wait(q_full, 0);
+  const uint64_t qdesc = make_sw128_desc(smem_u32(sQ + wg * (AT_Q_BYTES / 2)));
+#pragma unroll 1
+  for (int j = 0; j < ntiles; ++j) {
+    const int st = j % AT_ST, ph = (j / AT_ST) & 1;
+    // ---- S = Q . K''^T
+    float s[32];
+    mbar_wait(&k_full[st], ph);
+    {
+      const uint64_t kdesc = make_sw128_desc(smem_u32(sK + st * AT_TILE_BYTES));
+      wgmma_fence_regs<32>(s);
+      wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          umma_f16_ts(tmem_o, s_col(sb) + 8 * ks, vdesc + (uint64_t)(ks * ((16 * 128) >> 4)), idesc_pv, (cp.j | ks) != 0);
-        umma_commit(&s_empty[sb]);
-        umma_commit(&v_empty[vs]);
-        if (cp.j + 1 == cp.it.ntiles) umma_commit(o_done);
-        at_cursor_next(p, cp, n_items, nq);
-      };
-      // Every blocking wait below is on work this thread has ALREADY issued (or on the softmax warps, which only depend on
-      // issued work), so the single control thread can never wait for itself — also with one-tile items:
-      //   K''(n): needs QK(n - KST) issued  -> loaded while n - cq.n < KST - 1 (and the Q buffer is free, non-blocking);
-      //   V(n):   needs PV(n - VST) issued  -> loaded while n - cp.n < VST;
-      //   QK(n):  needs K''(n) requested and PV(n - NS) issued -> issued while n - cp.n < NS - 1 (one iteration of slack);
-      //   PV(n):  needs QK(n) issued and V(n) requested.
-      auto fill_k = [&]() {
-        while (ck.valid && ck.n - cq.n < ATP_KST - 1) {
-          if (!try_load_k()) break;
-        }
-      };
-      while (cp.valid) {
-        fill_k();
-        while (cv.valid && cv.n - cp.n < ATP_VST) load_v();
-        while (cq.valid && ck.n > cq.n && cq.n - cp.n < ATP_NS - 1) {
-          issue_qk();
-          fill_k();
-        }
-        if (cq.n > cp.n) issue_pv();
+      for (int k = 0; k < AT_DK / 16; ++k) wgmma_m64n64k16_ss(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs<32>(s);
+    }
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+    // ---- x = s * scale*log2e + key bias, masks, tile maximum per row
+    const int kbase = (jt0 + j) * AT_BN;
+    const float* bias = s_bias + j * AT_BN;
+    float tmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 b2 = *reinterpret_cast<const float2*>(bias + 8 * jj + cq);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        s[4 * jj + 2 * i] = fmaf(s[4 * jj + 2 * i], p.scale_log2, b2.x);
+        s[4 * jj + 2 * i + 1] = fmaf(s[4 * jj + 2 * i + 1], p.scale_log2, b2.y);
       }
     }
-  } else {
-    // ------------------------------------------------------------------ softmax warps: thread = query row
-    const int r = warp * 32 + lane;
-    const uint32_t lane_addr = ((uint32_t)(warp * 32) << 16);
-    constexpr int NB = 8;   // bias entries per thread and item (covers 16 key tiles = Tk <= 1024)
-    float bias_next[NB];
-    auto fetch_bias = [&](const AtItem& it, float(&dst)[NB]) {
-      const float* kb = p.key_bias ? p.key_bias + ((long long)it.g * p.H + it.h) * p.Tk : nullptr;
+    if (p.chunk > 0) {
 #pragma unroll
-      for (int i = 0; i < NB; ++i) {
-        const int kk = threadIdx.x + i * 128;
-        const int key = it.jt0 * 64 + kk;
-        dst[i] = (kk < it.ntiles * 64 && key < it.klen) ? (kb ? __ldg(kb + key) * p.scale_log2 : 0.f) : -INFINITY;
-      }
-    };
-    AtCursor c;
-    at_cursor_init(p, c, n_items, nq);
-    if (c.valid) fetch_bias(c.it, bias_next);
-    // items without a visible key (ntiles == 0) never enter the rings: their output rows are zero
-    auto zero_items_before = [&](int k_from, int k_to) {
-      for (int k = k_from; k < k_to; ++k) {
-        const long long id = (long long)blockIdx.x + (long long)k * gridDim.x;
-        if (id >= n_items) break;
-        const AtItem z = at_item(p, (int)id, nq);
-        const int row = z.q0 + r;
-        if (row < p.Tq) {
-          bf16* orow = p.out + ((long long)z.g * p.Tq + row) * p.ldo + z.h * AT_DK;
+      for (int i = 0; i < 2; ++i) {
+        const int lo = vis_lo(row[i]) - kbase, hi = vis_hi(row[i]) - kbase;   // visible columns: lo <= c < hi
 #pragma unroll
-          for (int q = 0; q < 8; ++q) reinterpret_cast<uint4*>(orow)[q] = make_uint4(0u, 0u, 0u, 0u);
-        }
-      }
-    };
-    zero_items_before(0, c.valid ? c.k : 0x7fffffff);
-    while (c.valid) {
-      const AtItem it = c.it;
-      const int k_this = c.k;
-      float* bias = s_bias + (c.ne & 1) * bias_len;
+        for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-      for (int i = 0; i < NB; ++i) {
-        const int kk = threadIdx.x + i * 128;
-        if (kk < it.ntiles * 64) bias[kk] = bias_next[i];
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // the four softmax warps: bias row of this item is complete
-      // next non-empty item's bias row: in flight during this item
-      AtCursor nx = c;
-      nx.j = it.ntiles - 1;
-      at_cursor_next(p, nx, n_items, nq);
-      if (nx.valid) fetch_bias(nx.it, bias_next);
-      float m_run = -INFINITY, row_sum = 0.f;
-      auto vis_lo = [&](int i) { return (p.chunk > 0 && p.left >= 0) ? max(0, (i / p.chunk - p.left) * p.chunk) : 0; };
-      auto vis_hi = [&](int i) { return p.chunk > 0 ? min(it.klen, (i / p.chunk + 1) * p.chunk) : it.klen; };
-      uint32_t sv[64];
-#pragma unroll 1
-      for (int j = 0; j < it.ntiles; ++j) {
-        const int n = c.n + j, sb = n % ATP_NS;
-        mbar_wait(&s_full[sb], (n / ATP_NS) & 1);
-        tc_fence_after();
-        tmem_ld_32x32(s_col(sb) + lane_addr, sv);
-        tmem_ld_32x32(s_col(sb) + lane_addr + 32, sv + 32);
-        tmem_ld_wait();
-        const uint32_t bias_addr = smem_u32(bias + j * 64);
-        float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        const float2 sc2 = make_float2(p.scale_log2, p.scale_log2);
-#pragma unroll
-        for (int e = 0; e < 64; e += 4) {
-          const float4 b4 = lds128(bias_addr + e * 4);
-          const float2 x01 = ffma2(make_float2(__uint_as_float(sv[e + 0]), __uint_as_float(sv[e + 1])), sc2,
-                                   make_float2(b4.x, b4.y));
-          const float2 x23 = ffma2(make_float2(__uint_as_float(sv[e + 2]), __uint_as_float(sv[e + 3])), sc2,
-                                   make_float2(b4.z, b4.w));
-          sv[e + 0] = __float_as_uint(x01.x);
-          sv[e + 1] = __float_as_uint(x01.y);
-          sv[e + 2] = __float_as_uint(x23.x);
-          sv[e + 3] = __float_as_uint(x23.y);
-          mx[(e >> 2) & 3] = fmax3(mx[(e >> 2) & 3], x01.x, x01.y);
-          mx[((e >> 2) + 2) & 3] = fmax3(mx[((e >> 2) + 2) & 3], x23.x, x23.y);
-        }
-        float tmax = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-        if (p.chunk > 0) {   // boundary tiles of the causal / chunk mask (see attention_tc_kernel)
-          const int kbase = (it.jt0 + j) * 64;
-          const int i0 = it.q0 + warp * 32;
-          if (kbase < vis_lo(i0 + 31) || kbase + 64 > vis_hi(i0)) {
-            const int lo = vis_lo(it.q0 + r) - kbase, hi = vis_hi(it.q0 + r) - kbase;
-            tmax = -INFINITY;
-#pragma unroll
-            for (int e = 0; e < 64; ++e) {
-              const float x = (e >= lo && e < hi) ? __uint_as_float(sv[e]) : -INFINITY;
-              sv[e] = __float_as_uint(x);
-              tmax = fmaxf(tmax, x);
-            }
+          for (int c = 0; c < 2; ++c) {
+            const int col = 8 * jj + cq + c;
+            if (col < lo || col >= hi) s[4 * jj + 2 * i + c] = -INFINITY;
           }
-        }
-        if (p.key_bits) {
-          const int kbase = (it.jt0 + j) * 64;
-          const uint32_t* mw =
-              p.key_bits + ((long long)it.g * p.Tq + min(it.q0 + r, p.Tq - 1)) * p.bits_ld + (kbase >> 5);
-          tmax = -INFINITY;
-#pragma unroll
-          for (int wi = 0; wi < 2; ++wi) {
-            const uint32_t word = __ldg(mw + wi);
-#pragma unroll
-            for (int e = 0; e < 32; ++e) {
-              const float x = ((word >> e) & 1u) ? __uint_as_float(sv[wi * 32 + e]) : -INFINITY;
-              sv[wi * 32 + e] = __float_as_uint(x);
-              tmax = fmaxf(tmax, x);
-            }
-          }
-        }
-        if (j == 0) {
-          m_run = tmax;
-        } else {
-          const bool raise = tmax > m_run + 8.f;
-          if (__any_sync(0xffffffffu, raise)) {
-            // lazy rescale: PV(n - 1) must have retired before O is touched
-            mbar_wait(&s_empty[(n - 1) % ATP_NS], ((n - 1) / ATP_NS) & 1);
-            tc_fence_after();
-            const float m_new = raise ? tmax : m_run;
-            const float f = (m_new == -INFINITY) ? 1.f : fast_exp2(m_run - m_new);
-            m_run = m_new;
-            row_sum *= f;
-#pragma unroll 1
-            for (int cc = 0; cc < 64; cc += 32) {
-              uint32_t ov[32];
-              tmem_ld_32x32(tmem_o + lane_addr + cc, ov);
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 32; ++e) ov[e] = __float_as_uint(__uint_as_float(ov[e]) * f);
-              tmem_st_32x32(tmem_o + lane_addr + cc, ov);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-          }
-        }
-        float2 sm01 = make_float2(0.f, 0.f), sm23 = make_float2(0.f, 0.f);
-        const float m_eff = (m_run == -INFINITY) ? 0.f : m_run;
-        const float2 one2 = make_float2(1.f, 1.f), negm2 = make_float2(-m_eff, -m_eff);
-#pragma unroll
-        for (int e = 0; e < 64; e += 4) {
-          const float2 d01 = ffma2(make_float2(__uint_as_float(sv[e + 0]), __uint_as_float(sv[e + 1])), one2, negm2);
-          const float2 d23 = ffma2(make_float2(__uint_as_float(sv[e + 2]), __uint_as_float(sv[e + 3])), one2, negm2);
-          float2 p01 = make_float2(fast_exp2(d01.x), fast_exp2(d01.y));
-          float2 p23 = make_float2(fast_exp2(d23.x), fast_exp2(d23.y));
-          // word i = keys (2i, 2i+1): overwrites consumed scores only
-          if (ATP_TRUNC) {
-            // P~ truncated to bf16 (byte permute), the row sum adds the same truncated values
-            const uint32_t b0 = __float_as_uint(p01.x) & 0xffff0000u, b1 = __float_as_uint(p01.y) & 0xffff0000u;
-            const uint32_t b2 = __float_as_uint(p23.x) & 0xffff0000u, b3 = __float_as_uint(p23.y) & 0xffff0000u;
-            sv[(e >> 1) + 0] = __byte_perm(b0, b1, 0x7632);
-            sv[(e >> 1) + 1] = __byte_perm(b2, b3, 0x7632);
-            p01 = make_float2(__uint_as_float(b0), __uint_as_float(b1));
-            p23 = make_float2(__uint_as_float(b2), __uint_as_float(b3));
-          } else {
-            // P~ rounded to nearest-even bf16 (one F2FP per pair), fp32 row sum of the unrounded values — measured 2.6 %
-            // faster than the truncation path (fewer ALU instructions; the softmax warps are latency / issue bound)
-            sv[(e >> 1) + 0] = pack_bf16x2(p01.x, p01.y);
-            sv[(e >> 1) + 1] = pack_bf16x2(p23.x, p23.y);
-          }
-          sm01 = ffma2(p01, one2, sm01);
-          sm23 = ffma2(p23, one2, sm23);
-        }
-        row_sum += (sm01.x + sm01.y) + (sm23.x + sm23.y);
-        tmem_st_32x32(s_col(sb) + lane_addr, sv);   // P~ row over the first 32 columns of its own S row
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[sb]);
       }
-      // ---- epilogue of the item: O / row_sum -> bf16 -> global
-      mbar_wait(o_done, c.ne & 1);
-      tc_fence_after();
-      const int row = it.q0 + r;
-      const float inv = row_sum > 0.f ? 1.f / row_sum : 0.f;
-      bf16* orow = p.out + ((long long)it.g * p.Tq + row) * p.ldo + it.h * AT_DK;
-#pragma unroll 1
-      for (int cc = 0; cc < 64; cc += 32) {
-        uint32_t ov[32];
-        tmem_ld_32x32(tmem_o + lane_addr + cc, ov);
-        tmem_ld_wait();
-        if (row < p.Tq) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(ov[8 * q + 0]) * inv, __uint_as_float(ov[8 * q + 1]) * inv);
-            u.y = pack_bf16x2(__uint_as_float(ov[8 * q + 2]) * inv, __uint_as_float(ov[8 * q + 3]) * inv);
-            u.z = pack_bf16x2(__uint_as_float(ov[8 * q + 4]) * inv, __uint_as_float(ov[8 * q + 5]) * inv);
-            u.w = pack_bf16x2(__uint_as_float(ov[8 * q + 6]) * inv, __uint_as_float(ov[8 * q + 7]) * inv);
-            reinterpret_cast<uint4*>(orow + cc)[q] = u;
-          }
-        }
-      }
-      tc_fence_before();   // the O reads above are ordered before this warp's next p_full arrival (PV(0) of the next item)
-      // advance to the next non-empty item (tile counter moves by this item's tiles)
-      c.j = it.ntiles - 1;
-      c.n += it.ntiles - 1;
-      at_cursor_next(p, c, n_items, nq);
-      zero_items_before(k_this + 1, c.valid ? c.k : 0x7fffffff);
     }
+    if (p.key_bits) {
+      // arbitrary visibility (prefix-tree self-attention: a node sees its ancestors): one bit per key of the row
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t* mw = p.key_bits + ((long long)g * p.Tq + min(row[i], p.Tq - 1)) * p.bits_ld + (kbase >> 5);
+        const uint32_t w0 = __ldg(mw), w1 = __ldg(mw + 1);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int col = 8 * jj + cq + c;
+            const uint32_t word = (col < 32) ? w0 : w1;
+            if (!((word >> (col & 31)) & 1u)) s[4 * jj + 2 * i + c] = -INFINITY;
+          }
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) tmax[i] = fmaxf(tmax[i], fmaxf(s[4 * jj + 2 * i], s[4 * jj + 2 * i + 1]));
+    // the four threads of a quad hold the same two rows
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      tmax[i] = fmaxf(tmax[i], __shfl_xor_sync(0xffffffffu, tmax[i], 1));
+      tmax[i] = fmaxf(tmax[i], __shfl_xor_sync(0xffffffffu, tmax[i], 2));
+    }
+    // ---- running maximum: O and the row sums move to the new maximum (rows without a visible key so far keep
+    // m = -inf and O = 0; exp2(-inf) = 0 gives them zero weights)
+    float m_eff[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float m_new = fmaxf(m_run[i], tmax[i]);
+      const float f = (m_new == -INFINITY || m_run[i] == m_new) ? 1.f : fast_exp2(m_run[i] - m_new);
+      m_run[i] = m_new;
+      row_sum[i] *= f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj + 2 * i] *= f;
+        o[4 * jj + 2 * i + 1] *= f;
+      }
+      m_eff[i] = (m_new == -INFINITY) ? 0.f : m_new;
+    }
+    // ---- P~ = exp2(x - m) rounded to bf16, packed as the A fragments of the PV product (k-step ks = keys
+    // [16ks, 16ks+16) = accumulator column groups 2ks and 2ks+1); the row sums add the same rounded values
+    uint32_t pa[16];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t w = pack_bf16x2(fast_exp2(s[4 * jj + 2 * i] - m_eff[i]), fast_exp2(s[4 * jj + 2 * i + 1] - m_eff[i]));
+        const float2 pr = unpack_bf16x2(w);
+        row_sum[i] += pr.x + pr.y;
+        pa[2 * jj + i] = w;   // ks = jj / 2: regs {jj even: a0 (row), a1 (row + 8); jj odd: a2, a3}
+      }
+    // ---- O += P~ . V
+    mbar_wait(&v_full[st], ph);
+    {
+      const uint64_t vdesc = make_sw128_desc(smem_u32(sV + st * AT_TILE_BYTES));
+      wgmma_fence_regs<32>(o);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < AT_BN / 16; ++ks)
+        wgmma_m64n64k16_rs_tb(o, pa + 4 * ks, vdesc + (uint64_t)((ks * 16 * 128) >> 4));   // 16 key rows of 128 B
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs<32>(o);
+    }
+    if (lane == 0) mbar_arrive(&v_empty[st]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+  // ---- epilogue: O / row_sum -> bf16 -> global (rows without a visible key: zeros)
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float sum = row_sum[i];
+    sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+    const float inv = sum > 0.f ? 1.f / sum : 0.f;
+    if (row[i] < p.Tq) {
+      bf16* orow = p.out + ((long long)g * p.Tq + row[i]) * p.ldo + h * AT_DK;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(orow + 8 * jj + cq) = pack_bf16x2(o[4 * jj + 2 * i] * inv, o[4 * jj + 2 * i + 1] * inv);
+    }
   }
 }
 
@@ -1085,32 +335,6 @@ relpos_prep_vec_kernel(const bf16* __restrict__ k, long long ldk, const bf16* __
   }
 }
 
-__global__ void relpos_vp_kernel(const bf16* __restrict__ pos, long long ldp, const float* __restrict__ bias_v,
-                                 float* __restrict__ vp, int T, int L, int H, int dk) {
-  // one warp per (l, h, t)
-  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (w >= (long long)L * H * T) return;
-  const int t = (int)(w % T), h = (int)((w / T) % H), l = (int)(w / ((long long)T * H));
-  const int d = H * dk;
-  const bf16* pr = pos + (long long)t * ldp + (long long)l * d + h * dk;
-  const float* v = bias_v + (long long)l * d + h * dk;
-  float acc = 0.f;
-  for (int c = lane; c < dk; c += 32) acc += v[c] * __bfloat162float(pr[c]);
-  acc = warp_sum(acc);
-  if (lane == 0) vp[w] = acc;
-}
-
-int launch_relpos_vp(const bf16* pos, int ldp, const float* bias_v_all, float* vp, int T, int L, int H, int dk,
-                     cudaStream_t stream) {
-  const long long warps = (long long)L * H * T;
-  if (warps <= 0) return 0;
-  relpos_vp_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, stream>>>(pos, ldp, bias_v_all, vp, T, L, H, dk);
-  RVB_COUNT_LAUNCH();
-  RVB_CHECK_LAUNCH();
-  return 0;
-}
-
 int launch_relpos_prep(const bf16* k, int ldk, const bf16* pos, int ldp, const float* bias_u, const float* bias_v,
                        bf16* kpp, float* cbias, int B, int T, int H, int dk, cudaStream_t stream) {
   RVB_REQUIRE(dk % 2 == 0, "relpos_prep: d_k must be even");
@@ -1168,11 +392,6 @@ int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
     RVB_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
     g_encode_att = reinterpret_cast<EncodeTiledFn>(fn);
   }
-  static int bn_sel = 0;
-  if (bn_sel == 0) {
-    const char* e = getenv("RVB_ATTN_BN");
-    bn_sel = (e && atoi(e) == 128) ? 128 : 64;
-  }
   AttnTcParams p;
   p.out = a.out;
   p.ldo = a.ldo;
@@ -1185,130 +404,18 @@ int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
   p.left = a.causal ? -1 : a.left_chunks;
   p.key_bits = a.key_bits;
   p.bits_ld = a.bits_ld;
-  {
-    static int pipe_sel = -1;
-    if (pipe_sel < 0) {
-      const char* e = getenv("RVB_ATTN_PIPE");
-      pipe_sel = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    p.pipe = pipe_sel;
-  }
   RVB_REQUIRE(a.key_bits == nullptr || a.bits_ld >= 2 * ((a.Tk + 63) / 64), "attention_tc: key_bits rows are too short");
   p.scale_log2 = a.scale * 1.4426950408889634f;
   CUtensorMap tmQ, tmK, tmV;
-  if (tmap_2d(&tmQ, a.q, (long long)a.H * AT_DK, (long long)a.groups * a.Tq, a.ldq, 128)) return -1;
-  if (tmap_2d(&tmK, a.k, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldk, bn_sel)) return -1;
-  if (tmap_2d(&tmV, a.v, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldv, bn_sel)) return -1;
+  if (tmap_2d(&tmQ, a.q, (long long)a.H * AT_DK, (long long)a.groups * a.Tq, a.ldq, AT_BM)) return -1;
+  if (tmap_2d(&tmK, a.k, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldk, AT_BN)) return -1;
+  if (tmap_2d(&tmV, a.v, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldv, AT_BN)) return -1;
   dim3 grid((a.Tq + AT_BM - 1) / AT_BM, a.H, a.groups);
-  static int sw_sel = 0;
-  if (sw_sel == 0) {
-    const char* e = getenv("RVB_ATTN_SW");
-    sw_sel = (e && atoi(e) == 8) ? 8 : 4;  // measured: 4 warps 0.388 ms / encoder layer, 8 warps 0.403 ms
-  }
-  // RVB_ATTN_PERSIST=1: the persistent kernel.  Correct (tests/test_gpu_kernels.py::...persistent_many_items...) but
-  // measured SLOWER than one item per CTA with P~ in tensor memory — 0.414 vs 0.330 ms per encoder layer, 0.029 vs
-  // 0.021 ms per key tile, the same 0.094 ms at one tile — so the per-item cost is the dependent chain Q -> S -> P~ -> O
-  // -> epilogue inside the softmax warps, not CTA launch / TMEM allocation / barrier setup, and the cursor bookkeeping
-  // lengthens the control thread's loop.  Default: off.
-  int persist_sel = 0;
-  {
-    const char* e = getenv("RVB_ATTN_PERSIST");   // read per call: the kernel test runs both variants in one process
-    persist_sel = (e && atoi(e) == 1) ? 1 : 0;
-  }
-  const bool plain_cfg = bn_sel == 64 && sw_sel == 4 && getenv("RVB_ATTN_POLY") == nullptr && getenv("RVB_ATTN_CW") == nullptr &&
-                         getenv("RVB_ATTN_PT") == nullptr;
-  if (persist_sel == 1 && plain_cfg && a.Tk <= 1024) {
-    int dev = 0, sms = 0;
-    RVB_CHECK_CUDA(cudaGetDevice(&dev));
-    RVB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const int nq = (a.Tq + AT_BM - 1) / AT_BM;
-    const long long n_items = (long long)nq * a.H * a.groups;
-    RVB_REQUIRE(n_items < (1ll << 31), "attention_tc: too many work items");
-    const int bias_len = ((a.Tk + 63) / 64) * 64;
-    const size_t smem = ATP_SMEM_FIXED + (size_t)2 * bias_len * sizeof(float);
-    static DynSmemOptIn optin_p;
-    if (optin_p.ensure(attention_tcp_kernel, smem)) return -1;
-    const int ctas = (int)std::min<long long>(n_items, 2ll * sms);
-    attention_tcp_kernel<<<ctas, 160, smem, stream>>>(tmQ, tmK, tmV, p, (int)n_items, nq, bias_len);
-    RVB_COUNT_LAUNCH();
-    RVB_CHECK_LAUNCH();
-    return 0;
-  }
-  if (bn_sel == 128) {
-    const size_t smem = AtCfg<128>::SMEM_FIXED + (size_t)((a.Tk + 127) / 128) * 128 * sizeof(float);
-    RVB_REQUIRE(smem <= 227 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
-    static DynSmemOptIn optin;
-    if (optin.ensure(attention_tc_kernel<128, 4, 0>, smem)) return -1;
-    attention_tc_kernel<128, 4, 0><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-  } else if (sw_sel == 4) {
-    const size_t smem = AtCfg<64>::SMEM_FIXED + (size_t)((a.Tk + 63) / 64) * 64 * sizeof(float);
-    RVB_REQUIRE(smem <= 113 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
-    static int poly_sel = -1;   // RVB_ATTN_POLY=0|1|2: share of the exponentials on the FMA pipe (0 none, 1 half, 2 quarter)
-    if (poly_sel < 0) {
-      const char* e = getenv("RVB_ATTN_POLY");
-      poly_sel = e ? atoi(e) : 0;
-      if (poly_sel < 0 || (poly_sel > 3 && poly_sel < 8) || poly_sel > 17) poly_sel = 0;
-    }
-    static DynSmemOptIn optin[3];
-    static DynSmemOptIn optin_abl[10];
-    static DynSmemOptIn optin_rn;
-    if (poly_sel == 3) {   // P~ rounded by F2FP instead of truncated (A/B), P~ in tensor memory
-      if (optin_rn.ensure(attention_tc_kernel<64, 4, 3, false, true>, smem)) return -1;
-      attention_tc_kernel<64, 4, 3, false, true><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-    } else if (poly_sel >= 8) {   // timing ablations, wrong results (see the kernel)
-#define RVB_ABL(V)                                                                     \
-  do {                                                                                 \
-    if (optin_abl[V - 8].ensure(attention_tc_kernel<64, 4, V>, smem)) return -1;       \
-    attention_tc_kernel<64, 4, V><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);      \
-  } while (0)
-      if (poly_sel == 8) RVB_ABL(8);
-      else if (poly_sel == 9) RVB_ABL(9);
-      else if (poly_sel == 10) RVB_ABL(10);
-      else if (poly_sel == 11) RVB_ABL(11);
-      else if (poly_sel == 12) RVB_ABL(12);
-      else if (poly_sel == 13) RVB_ABL(13);
-      else if (poly_sel == 14) RVB_ABL(14);
-      else if (poly_sel == 15) RVB_ABL(15);
-      else if (poly_sel == 16) RVB_ABL(16);
-      else RVB_ABL(17);
-#undef RVB_ABL
-    } else
-    if (poly_sel == 1) {
-      if (optin[1].ensure(attention_tc_kernel<64, 4, 1>, smem)) return -1;
-      attention_tc_kernel<64, 4, 1><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-    } else if (poly_sel == 2) {
-      if (optin[2].ensure(attention_tc_kernel<64, 4, 2>, smem)) return -1;
-      attention_tc_kernel<64, 4, 2><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-    } else {
-      static int cw_sel = -1;   // RVB_ATTN_CW=3: three control warps (measured slower: 0.481 vs 0.435 ms); default: one thread
-      if (cw_sel < 0) {
-        const char* e = getenv("RVB_ATTN_CW");
-        cw_sel = (e && atoi(e) == 3) ? 3 : 1;
-      }
-      static int pt_sel = -1;   // RVB_ATTN_PT=0: P~ through shared memory (A/B); default: P~ in tensor memory
-      if (pt_sel < 0) {
-        const char* e = getenv("RVB_ATTN_PT");
-        pt_sel = (e && atoi(e) == 0) ? 0 : 1;
-      }
-      static DynSmemOptIn optin_cw3, optin_pt;
-      if (cw_sel != 3 && pt_sel == 1) {
-        if (optin_pt.ensure(attention_tc_kernel<64, 4, 0, false, true>, smem)) return -1;
-        attention_tc_kernel<64, 4, 0, false, true><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-      } else if (cw_sel == 3) {
-        if (optin_cw3.ensure(attention_tc_kernel<64, 4, 0, true>, smem)) return -1;
-        attention_tc_kernel<64, 4, 0, true><<<grid, 256, smem, stream>>>(tmQ, tmK, tmV, p);
-      } else {
-        if (optin[0].ensure(attention_tc_kernel<64, 4, 0>, smem)) return -1;
-        attention_tc_kernel<64, 4, 0><<<grid, 160, smem, stream>>>(tmQ, tmK, tmV, p);
-      }
-    }
-  } else {
-    const size_t smem = AtCfg<64>::SMEM_FIXED + 3072 + (size_t)((a.Tk + 63) / 64) * 64 * sizeof(float);
-    RVB_REQUIRE(smem <= 113 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
-    static DynSmemOptIn optin;
-    if (optin.ensure(attention_tc_kernel<64, 8, 0>, smem)) return -1;
-    attention_tc_kernel<64, 8, 0><<<grid, 288, smem, stream>>>(tmQ, tmK, tmV, p);
-  }
+  const size_t smem = AT_SMEM_FIXED + (size_t)((a.Tk + AT_BN - 1) / AT_BN) * AT_BN * sizeof(float);
+  RVB_REQUIRE(smem <= 227 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
+  static DynSmemOptIn optin;
+  if (optin.ensure(attention_tc_kernel, smem)) return -1;
+  attention_tc_kernel<<<grid, AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
   return 0;

@@ -849,7 +849,7 @@ trie_inputs_kernel(const int* __restrict__ node_of, int nstride, const int* __re
   const int* ndep = node_dep + (size_t)b * cap;
   for (int node = threadIdx.x; node < P; node += blockDim.x) {
     const size_t r = (size_t)b * P + node;
-    if (anc_bits) {  // the same ancestor set as a bit row over the utterance's node slots (tcgen05 attention mask)
+    if (anc_bits) {  // the same ancestor set as a bit row over the utterance's node slots (wgmma attention mask)
       uint32_t* br = anc_bits + r * bits_ld;
       for (int w = 0; w < bits_ld; ++w) br[w] = 0u;
       int cur = node;

@@ -1,13 +1,13 @@
-// reverb_b200 — speaker-embedding network of the diarization pipeline (WeSpeaker ResNet34) on sm_100a.
+// reverb_b200 — speaker-embedding network of the diarization pipeline (WeSpeaker ResNet34) on sm_90a.
 //
 // Replaces `pyannote.audio` `WeSpeakerResNet34.forward(waveforms, weights)` behind
-// `Pipeline.from_pretrained('Revai/reverb-diarization-v1')` (/root/reference/diarization/infer_pyannote3.0.py:33-40).
+// `Pipeline.from_pretrained('Revai/reverb-diarization-v1')` (reference: diarization/infer_pyannote3.0.py:33-40).
 // ** parity unpinned ** — see include/rvb_diar.h.
 //
 //   window in [-1, 1] -> x 2^15 -> Kaldi fbank (fbank.cu, hamming window) -> minus the mean over time
 //   -> conv 3x3 (1 -> C) + BN + ReLU                                   direct kernel, fp32 input
 //   -> 16 BasicBlocks: [conv 3x3 (stride s) + BN + ReLU, conv 3x3 + BN, (+ 1x1 stride-s conv + BN shortcut), add, ReLU]
-//      every 3x3 / 1x1 convolution = im2col (bf16, NHWC, K ordered (kh, kw, c)) + the tcgen05 GEMM of gemm.cu with the
+//      every 3x3 / 1x1 convolution = im2col (bf16, NHWC, K ordered (kh, kw, c)) + the wgmma GEMM of gemm.cu with the
 //      BatchNorm folded into its weights / bias and ReLU in its epilogue; the residual add reads the GEMM's fp32 output
 //   -> weighted statistics pooling over time per (channel, frequency) -> Linear(embed_dim) in fp32
 //
@@ -424,7 +424,7 @@ RVB_API int rvb_emb_forward(rvb_emb_model* m, const float* d_wave, int B, int nu
   // front-end
   {
     const long long n = (long long)B * num_samples;
-    scale_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 148 * 16), 256, 0, stream>>>(d_wave, m->ws_wave.as<float>(), n,
+    scale_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 132 * 16), 256, 0, stream>>>(d_wave, m->ws_wave.as<float>(), n,
                                                                                            32768.f);
     RVB_COUNT_LAUNCH();
     RVB_CHECK_LAUNCH();

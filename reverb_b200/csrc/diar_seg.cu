@@ -1,7 +1,7 @@
-// reverb_b200 — segmentation network of the diarization pipeline (PyanNet) on sm_100a, fp32.
+// reverb_b200 — segmentation network of the diarization pipeline (PyanNet) on sm_90a, fp32.
 //
 // Replaces `pyannote.audio` `PyanNet.forward` behind `Pipeline.from_pretrained('Revai/reverb-diarization-v1')`
-// (/root/reference/diarization/infer_pyannote3.0.py:33-40).  ** parity unpinned ** — see include/rvb_diar.h.
+// (reference: diarization/infer_pyannote3.0.py:33-40).  ** parity unpinned ** — see include/rvb_diar.h.
 //
 //   waveform window (B, N) -> InstanceNorm1d(1) -> SincNet:  |sinc band-pass bank (80 x 251, stride 10)| -> MaxPool(3)
 //   -> InstanceNorm -> LeakyReLU -> 2 x [Conv1d(k=5) -> MaxPool(3) -> InstanceNorm -> LeakyReLU]      (B, frames, 60)

@@ -638,9 +638,9 @@ int launch_conv_mid(const bf16* x, const float* pad_glu, const float* dw_w, cons
                                                    conv_tmp, stats, out, T, C, K, causal, conv_chunk)
   RVB_REQUIRE(conv_chunk <= 0 || !causal, "conv_mid: chunk-local convolution is the non-causal streaming mode");
   {
-    // RVB_CONV_FUSED=1: the single-kernel variant.  Measured SLOWER at the benchmark shape (0.226 ms vs 0.094 + 0.059 ms
-    // per layer, profiles/r2f_launches_summary.md): 512 threads x 98 registers leave one CTA per SM and the three phases
-    // (taps, statistics, normalise) run back to back instead of overlapping across CTAs.  Kept as an option.
+    // RVB_CONV_FUSED=1: the single-kernel variant (not the default): 512 threads x 98 registers leave one CTA per SM and
+    // the three phases (taps, statistics, normalise) run back to back instead of overlapping across CTAs.  Kept as an
+    // option; not timed on the H100.
     static int fused_sel = -1;
     if (fused_sel < 0) {
       const char* e = getenv("RVB_CONV_FUSED");
@@ -706,7 +706,7 @@ __global__ void scale_cast_kernel(const float* __restrict__ x, float scale, floa
 int launch_scale_cast(const float* x, float scale, float* out_f32, bf16* out_bf16, long long n, cudaStream_t stream) {
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   scale_cast_kernel<<<(int)blocks, 256, 0, stream>>>(x, scale, out_f32, out_bf16, n);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
@@ -735,7 +735,7 @@ int launch_f32_to_pair(const float* x, bf16* out, long long rows, int width, cud
   const long long n = rows * width;
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   f32_to_pair_kernel<<<(int)blocks, 256, 0, stream>>>(x, out, rows, width);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
@@ -767,7 +767,7 @@ int launch_weighted_sum_bf16(const float* const* ins, const float* coef, int n_i
     w.c[i] = coef[i];
   }
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   weighted_sum_kernel<<<(int)blocks, 256, 0, stream>>>(w, n_in, n, out_bf16, out_f32);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();

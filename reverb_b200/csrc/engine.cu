@@ -157,7 +157,6 @@ struct rvb_model {
   Linear conv2;    // (d, 9*d) ordered (kh, kw, c)
   Linear embed;    // (d, F2*d) ordered (f, c), scaled by sqrt(d)
   Linear pos_all;  // (L*d, d) stacked linear_pos weights, no bias
-  float* pos_v_all = nullptr;  // (L, d) stacked pos_bias_v (for the input-independent v . pos table)
   std::vector<EncLayer> enc;
   Norm after_norm;
   Linear ctc;
@@ -172,9 +171,8 @@ struct rvb_model {
   DevBuf ws_encbf, ws_logits, ws_dec[12], ws_search, ws_misc, ws_kpp, ws_cbias;
   HostPinned pin_a, pin_b, pin_c, pin_d, pin_e;
   int pe_T = 0;
-  int pall_T = 0;               // ws_pall / ws_vp hold linear_pos(pos_emb) and v . pos for this many frames
+  int pall_T = 0;               // ws_pall holds linear_pos(pos_emb) for this many frames
   const void* pall_ptr = nullptr;
-  DevBuf ws_vp;
   int lens_slot = 0;
   int lens_B = 0;
   static constexpr int kTickets = 4;
@@ -418,7 +416,7 @@ static int finalize_model(rvb_model* m) {
   }
   if (load_norm(m, "encoder.after_norm", d, &m->after_norm)) return -1;
   m->enc.resize(L);
-  std::vector<float> posw, posv;
+  std::vector<float> posw;
   for (int i = 0; i < L; ++i) {
     EncLayer& E = m->enc[i];
     const std::string p = "encoder.encoders." + std::to_string(i);
@@ -438,7 +436,6 @@ static int finalize_model(rvb_model* m) {
     posw.insert(posw.end(), t->begin(), t->end());
     if (need(m, p + ".self_attn.pos_bias_u", d, &t) || upload_f32(m, t->data(), d, &E.pos_u)) return -1;
     if (need(m, p + ".self_attn.pos_bias_v", d, &t) || upload_f32(m, t->data(), d, &E.pos_v)) return -1;
-    posv.insert(posv.end(), t->begin(), t->end());
     if (load_linear_glu(m, p + ".conv_module.pointwise_conv1", d, d, &E.pw1, &E.pad_glu) ||
         load_linear(m, p + ".conv_module.pointwise_conv2", d, d, &E.pw2))
       return -1;
@@ -456,7 +453,6 @@ static int finalize_model(rvb_model* m) {
   if (upload_w(m, posw.data(), (size_t)L * d, d, &m->pos_all.w)) return -1;
   m->pos_all.N = L * d;
   m->pos_all.K = d;
-  if (upload_f32(m, posv.data(), posv.size(), &m->pos_v_all)) return -1;
   if (load_linear(m, "ctc.ctc_lo", c.vocab, d, &m->ctc)) return -1;
   if (c.dec_blocks > 0 && find_host(m, "decoder.left_decoder.embed.0.weight")) {
     if (load_decoder(m, "left_decoder", c.dec_blocks, &m->dec_l)) return -1;
@@ -522,7 +518,7 @@ static int gemm(rvb_model* m, const bf16* A, const Linear& W, int M, int act, in
   return launch_gemm(g, stream);
 }
 
-// 1 = tcgen05 attention (default when d_k == 64), 0 = mma.sync kernel (RVB_ATTN=mma)
+// 1 = wgmma attention (default when d_k == 64), 0 = mma.sync kernel (RVB_ATTN=mma)
 static int attn_impl() {
   static int v = -1;
   if (v < 0) {
@@ -575,14 +571,14 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
       m->ws_att.ensure((size_t)M * d * 2 * pm) || m->ws_pw.ensure((size_t)M * d * 2 * pm) ||
       m->ws_cm.ensure((size_t)M * d * 2 * pm) || m->ws_y.ensure((size_t)M * d * 4) ||
       m->ws_ybf.ensure((size_t)M * d * 2 * pm) || m->ws_pall.ensure((size_t)Tp * L * d * 2 * pm) ||
-      m->ws_kpp.ensure((size_t)M * d * 2) || m->ws_vp.ensure((size_t)L * H * Tp * sizeof(float)) ||
+      m->ws_kpp.ensure((size_t)M * d * 2) ||
       m->ws_cbias.ensure(((size_t)B * H * Tp + (size_t)M * 2 * ((d / 2 + 127) / 128)) * 4))
     return -1;
   const bool tc_attn = attn_impl() == 1 && dk == 64 && !x3;
   if (!tc_attn && !x3 && attn_impl() == 1) {   // say so once: a d_k != 64 model runs the (slower) mma.sync attention
     static std::atomic<bool> warned{false};
     if (!warned.exchange(true))
-      fprintf(stderr, "reverb_b200: d_k = %d — the tcgen05 attention kernel is built for d_k = 64; using the mma.sync kernel\n", dk);
+      fprintf(stderr, "reverb_b200: d_k = %d — the wgmma attention kernel is built for d_k = 64; using the mma.sync kernel\n", dk);
   }
   // rel-pos key transform inside the [q; k; v] projection's epilogue (default); RVB_RELPOS=prep keeps the separate kernel
   const char* rp_env = getenv("RVB_RELPOS");   // read per call: tests A/B the two paths in one process
@@ -614,11 +610,10 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     }
     m->pe_T = Tp;
   }
-  // ... which depends on the frame count only: kept across calls of the same shape, with the table v_h . pos[t]
+  // ... which depends on the frame count only: kept across calls of the same shape
   if (m->pall_T != Tp || m->pall_ptr != (const void*)pall) {
     if (gemm(m, m->ws_pe.as<bf16>(), m->pos_all, Tp, ACT_NONE, OUT_BF16, pall, 1.f, stream, nullptr, 0, 0, false))
       return -1;
-    if (!x3 && launch_relpos_vp(pall, L * d, m->pos_v_all, m->ws_vp.as<float>(), Tp, L, H, dk, stream)) return -1;
     m->pall_T = Tp;
     m->pall_ptr = pall;
   }
@@ -683,7 +678,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
       g.rp_H = H;
       g.rp_col0 = d;
       g.rp_u = E.pos_u;
-      g.rp_vp = m->ws_vp.as<float>() + (size_t)l * H * Tp;
+      g.rp_v = E.pos_v;
       g.rp_cb = m->ws_cbias.as<float>();
       if (launch_gemm(g, stream)) return -1;
     } else if (gemm(m, n, E.qkv, (int)M, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) {
@@ -742,7 +737,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
       a.scale = att_scale;
       if (launch_attention_tc(a, stream)) return -1;
     } else {
-      RVB_REQUIRE(att_chunk <= 0, "encoder_forward: chunk-masked attention needs the tcgen05 kernel (d_k = 64)");
+      RVB_REQUIRE(att_chunk <= 0, "encoder_forward: chunk-masked attention needs the wgmma kernel (d_k = 64)");
       AttnArgs a;
       a.q = qkv;
       a.k = qkv + d;
@@ -1292,7 +1287,7 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
   const size_t pm = (size_t)m->pm();
   const int ldv = (V + 3) & ~3;
   DevBuf* w = m->ws_dec;
-  // bf16 mode: self-attention of the tree on the tcgen05 kernel (dense over the utterance's P node slots, causal tile
+  // bf16 mode: self-attention of the tree on the wgmma kernel (dense over the utterance's P node slots, causal tile
   // range — a parent always precedes its children — plus an ancestor bit mask); accurate mode: fp32 over ancestor lists
   const bool tc_self = !x3 && attn_impl() == 1 && dk == 64 && !(getenv("RVB_TRIE_ATTN") && strcmp(getenv("RVB_TRIE_ATTN"), "list") == 0);
   const int bits_ld = 2 * ((P + 63) / 64);
@@ -1533,7 +1528,7 @@ static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* 
 
 // ctc_prefix_beam_search + attention_rescoring with the n-best kept on the device in between (asr_model.py:259-308 does
 // the same two steps through Python lists), split into three host calls around a TICKET so that consecutive batches
-// can be software-pipelined on one stream by one host thread (VERDICT r1 "GPU idle 9.7 ms/step"):
+// can be software-pipelined on one stream by one host thread (no GPU idle time while the host picks the decoder batch):
 //   search_submit     enqueue the prefix beam search + the small D2H copy (hypothesis lengths / counts / CTC scores)
 //   rescoring_submit  wait for that copy (the ONLY data-dependent host decision of the path: the decoder batch is
 //                     padded to the longest hypothesis), enqueue decoder-input assembly, the decoder passes and the
@@ -1616,7 +1611,7 @@ static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val,
   int* hp_small = t.small.as<int>();
   int* hp_elen = reinterpret_cast<int*>(reinterpret_cast<char*>(hp_small) + t.small_bytes);
   memcpy(hp_elen, h_enc_lens, sizeof(int) * B);
-  // The search runs on a SIDE stream: it is one CTA per utterance (64 of 148 SMs, latency-bound, ~2.7 ms at B = 64), so
+  // The search runs on a SIDE stream: it is one CTA per utterance (64 of 132 SMs, latency-bound), so
   // in a pipelined decode the next batch's fbank / conv1 (bandwidth-bound, small CTAs) share the GPU with it instead of
   // queueing behind it.  The side stream starts after everything enqueued so far on `stream` (the CTC top-k);
   // rescoring_submit makes `stream` wait for ev_search before it touches the n-best.
@@ -1833,7 +1828,6 @@ RVB_API rvb_model* rvb_model_fork(rvb_model* m) {
   f->conv2 = m->conv2;
   f->embed = m->embed;
   f->pos_all = m->pos_all;
-  f->pos_v_all = m->pos_v_all;
   f->enc = m->enc;
   f->after_norm = m->after_norm;
   f->ctc = m->ctc;
@@ -1867,7 +1861,7 @@ RVB_API void rvb_model_destroy(rvb_model* m) {
   for (void* p : m->owned) cudaFree(p);
   DevBuf* bufs[] = {&m->ws_c1, &m->ws_c2, &m->ws_x, &m->ws_n, &m->ws_h, &m->ws_qkv, &m->ws_att, &m->ws_pw, &m->ws_cm,
                     &m->ws_y, &m->ws_ybf, &m->ws_pe, &m->ws_pall, &m->ws_lens, &m->ws_encbf, &m->ws_logits,
-                    &m->ws_search, &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold, &m->ws_vp};
+                    &m->ws_search, &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold};
   for (DevBuf* b : bufs) b->release();
   for (auto& b : m->ws_dec) b.release();
   if (m->tickets) {

@@ -1,4 +1,4 @@
-// reverb_b200 — Kaldi-compatible 80-bin log-mel filterbank, one fused kernel (sm_100a).
+// reverb_b200 — Kaldi-compatible 80-bin log-mel filterbank, one fused kernel (sm_90a).
 //
 // Replaces `torchaudio.compliance.kaldi.fbank(waveform, num_mel_bins=80, frame_length=25, frame_shift=10,
 // dither=0.0, energy_floor=0.0, sample_frequency=16000)` as called by the reference at
@@ -149,7 +149,7 @@ __device__ __forceinline__ void dft8(float2* a) {
 // itself is 8 x 8 x 4 (Cooley-Tukey): two 8-point DFTs in REGISTERS per lane with one shared-memory exchange between
 // them (conflict-free padded layout), the last radix-4 step across the 4 neighbouring lanes with shuffles.  Per frame and lane:
 // 16 + 16 shared-memory accesses for the FFT instead of the 360 of a radix-2 shared-memory FFT on the full 512
-// complex points (the round-1 kernel: 1.70 ms per 64 x 30 s; VERDICT r1 "fbank at 0.7 % of the HBM roofline").
+// complex points.
 //   n = 32 n1 + n2, k = k1 + 8 k2:   Z[k1 + 8 k2] = sum_n2 W256^(n2 k1) W32^(n2 k2) [ sum_n1 z[32 n1 + n2] W8^(n1 k1) ]
 //   n2 = 4 a + b,   k2 = c + 8 d:    (32-point)   = sum_b W32^(b c) W4^(b d)   [ sum_a  y[4 a + b]     W8^(a c)  ]
 constexpr int FB_FPW = 4;      // frames per warp

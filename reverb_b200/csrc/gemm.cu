@@ -1,6 +1,6 @@
-// reverb_b200 — persistent, warp-specialised tcgen05 + TMA GEMM for sm_100a.
+// reverb_b200 — persistent, warp-specialised wgmma + TMA GEMM for sm_90a.
 //
-//   C[M,N] = A[M,K] . W[N,K]^T  (+bias, activation, residual)      A, W: bf16, K-major; fp32 accumulate in TMEM
+//   C[M,N] = A[M,K] . W[N,K]^T  (+bias, activation, residual)      A, W: bf16, K-major; fp32 accumulate
 //
 // One kernel serves every dense layer on the hot path: the Conformer FFN / attention projections / pointwise convs
 // (reference: asr/wenet/transformer/positionwise_feed_forward.py:47-55, attention.py:52-79, convolution.py:129,139),
@@ -8,22 +8,15 @@
 // Conv2d(d,d,3,stride 2) of Conv2dSubsampling4 (subsampling.py:186-189) as an implicit GEMM whose A tiles are fetched
 // straight out of the channels-last conv1 activation by 4-D TMA boxes (no im2col buffer).
 //
-// Structure per CTA (320 threads, 1 CTA / SM, grid = #SMs, static round-robin tile scheduler):
-//   warp 0 / lane 0 : TMA producer   — fills a STAGES-deep ring of {A 128x64, W tile} bf16 tiles (SWIZZLE_128B)
-//   warp 1 / lane 0 : MMA issuer     — tcgen05.mma kind::f16, K=16 x 4 per stage; tcgen05.commit frees smem stages and
-//                                       publishes finished accumulators
-//   warps 2..9      : epilogue       — tcgen05.ld 32x32b from a double-buffered TMEM accumulator (2 x BN columns),
-//                                       bias / ReLU / SiLU / GLU / residual(+row mask) fused; outputs pass through a
-//                                       warp-private XOR-swizzled staging tile so global accesses are coalesced
-// so tile i's epilogue overlaps tile i+1's main loop.
-//   gemm_tc2_kernel (default): a CLUSTER of two CTAs works on a 256 x BN tile with tcgen05.mma.cta_group::2 — each
-//     CTA loads its own 128 A rows and HALF of the W tile, the leader CTA issues the MMAs for both, commits are
-//     multicast to both CTAs' barriers; both CTAs run epilogue warps on their own 128 accumulator rows.
-//   gemm_tc_kernel (RVB_GEMM=tc1): the single-CTA version, M = 128 per tile.
-// Tuning aids (environment, read once): RVB_GEMM_EPI_WARPS=4|8, RVB_GEMM_SKIP_EPI=1|2|3 (main loop only / no global
-// stores / TMEM loads + math only — results are wrong by construction; tools/gemm_bench.py).  Measured on the FFN-w1
-// shape (M=47872, N=4096, K=1024, bf16+SiLU): main loop alone 1696 TFLOP/s, + TMEM loads and math 1548, + staging
-// 1416, + global stores 1353 (cuBLAS without activation: 1450).
+// Structure per CTA (288 threads, 1 CTA / SM, grid = #SMs, static round-robin tile scheduler), see gemm_wg_kernel:
+//   warp 8 / lane 0 : TMA producer — fills a 4-deep ring of {A 128x64, W BNx64} bf16 tiles (SWIZZLE_128B)
+//   warps 0..7      : two consumer warpgroups, 64 rows each: wgmma m64nBNk16 from shared memory into registers, then
+//                     the fused epilogue (bias / ReLU / SiLU / GLU / residual(+row mask) / log-sum-exp / rel-pos keys)
+//                     on a shared-memory copy of the accumulator; outputs pass through a warp-private XOR-swizzled
+//                     staging tile so global accesses are coalesced.
+// Tuning aid (environment, read once): RVB_GEMM_SKIP_EPI=1|2|3 (main loop only / no global stores / accumulator
+// reads + math only — results are wrong by construction; tools/gemm_bench.py).  RVB_GEMM=simt selects the CUDA-core
+// bring-up kernel, RVB_GEMM=narrow 64-wide tiles wherever the epilogue allows them.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -40,8 +33,8 @@ void set_gemm_impl(int impl) { g_gemm_impl = impl; }
 int get_gemm_impl() {
   if (g_gemm_impl < 0) {
     const char* e = getenv("RVB_GEMM");
-    // default: 2-CTA (cta_group::2) kernel; RVB_GEMM=tc1 -> 1-CTA kernel, RVB_GEMM=simt -> CUDA-core bring-up kernel
-    g_gemm_impl = (e && strcmp(e, "simt") == 0) ? 1 : (e && strcmp(e, "tc1") == 0) ? 0 : 2;
+    // default: wgmma kernel; RVB_GEMM=simt -> CUDA-core bring-up kernel, RVB_GEMM=narrow -> wgmma with 64-wide tiles
+    g_gemm_impl = (e && strcmp(e, "simt") == 0) ? 1 : (e && strcmp(e, "narrow") == 0) ? 2 : 0;
   }
   return g_gemm_impl;
 }
@@ -66,7 +59,7 @@ struct GemmKParams {
   long long rp_ldp;
   int rp_T, rp_H, rp_col0;
   const float* rp_u;
-  const float* rp_vp;
+  const float* rp_v;
   float* rp_cb;
   int x3;              // bf16x3 accurate mode: num_k_blocks = 3 * kb_seg, pass s reads A half (s == 1), W half (s == 2)
   int kb_seg;          // k-blocks per pass (K / 64)
@@ -77,7 +70,6 @@ struct GemmKParams {
   int glu_coalesced;   // ACT_GLU with 16-byte aligned output rows (always true after the launch checks)
   int bf16_coalesced;  // bf16 output rows are 16-byte aligned -> staged, coalesced epilogue (see drain_tile)
   int f32_coalesced;  // fp32 output rows are 16-byte aligned -> staged, coalesced epilogue (see drain_tile)
-  int epi_warps;  // 4 or 8 epilogue warps drain a tile (8: short-K, epilogue-bound shapes; 4: long-K, MMA-bound)
   // simt fallback only
   const bf16* A;
   const bf16* W;
@@ -284,8 +276,24 @@ __device__ __forceinline__ long long output_row(const GemmKParams& p, const Tile
   return m;
 }
 
-// Drains columns [c0, c1) of one accumulator stage for the 32 output rows of one epilogue warp (one thread = one TMEM
-// lane = one row after tcgen05.ld).  Waits for the accumulator first.
+// The accumulator tile is copied from the wgmma fragments to shared memory as fp32 [BM][BN] with the 16-byte chunks of
+// row r XOR-swizzled by r % 8: the fragment stores (8 rows x 32 bytes per instruction) and the row reads below (32 rows
+// x 16 bytes) both spread over all banks.  One thread reads 32 consecutive columns [c, c+32) of its row (c % 32 == 0).
+template <int BN>
+__device__ __forceinline__ void acc_ld32(const float* accs, int row, int c, uint32_t* r) {
+  const float* rp = accs + row * BN;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float4 v = *reinterpret_cast<const float4*>(rp + ((((c >> 2) + k) ^ (row & 7)) << 2));
+    r[4 * k + 0] = __float_as_uint(v.x);
+    r[4 * k + 1] = __float_as_uint(v.y);
+    r[4 * k + 2] = __float_as_uint(v.z);
+    r[4 * k + 3] = __float_as_uint(v.w);
+  }
+}
+
+// Drains columns [c0, c1) of the accumulator tile for the 32 output rows of one epilogue warp (one thread = one row,
+// read from the tile's shared-memory copy, see acc_ld32).  The caller has synchronised the tile.
 //
 // fp32 outputs (EPI_F32, EPI_RESID) go through a warp-private 32x32 fp32 staging tile in shared memory (XOR-swizzled
 // in 16-byte slots, conflict-free both ways) so that global accesses are coalesced: one warp instruction covers 4 rows
@@ -295,22 +303,17 @@ __device__ __forceinline__ long long output_row(const GemmKParams& p, const Tile
 // accumulator barrier and chunk c+1's while chunk c is being converted.
 // PAIR (compile time): bf16 outputs are written as the accurate mode's (hi, lo) pair, lo at column + p.out_split, and
 // SiLU / GLU use exact exp / division — kept out of the throughput kernels (PAIR = false) so that their epilogue is the
-// straight-line code it was before the accurate mode existed (a run-time flag cost the SiLU GEMM 28 %).
-template <int EPI, bool PAIR>
-__device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord& t, int q, int lane, uint32_t taddr,
-                                           int c0, int c1, uint64_t* tfull_bar, uint32_t aphase, float* stage) {
-  const long long orow = output_row(p, t, q * 32 + lane);
+// straight-line code it was before the accurate mode existed (a run-time flag adds work to every element).
+template <int BN, int EPI, bool PAIR>
+__device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord& t, int q, int lane, const float* accs,
+                                           int c0, int c1, float* stage) {
+  const int arow = q * 32 + lane;
+  const long long orow = output_row(p, t, arow);
   const int n0_tile = t.n0;
-  if (p.debug_skip_epi == 1) {  // main-loop-only timing: wrong results by construction (2: everything but the stores)
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
-    return;
-  }
+  if (p.debug_skip_epi == 1) return;  // main-loop-only timing: wrong results by construction (2: everything but the stores)
   if constexpr (EPI == EPI_LSE) {
     // log-sum-exp partial of x = acc + bias over this thread's columns [c0, c1) of the tile (one 128-column slab when
     // 8 warps drain a 256-wide tile, two slabs with 4 warps) + the gather target if it falls inside
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
     const int g = (orow >= 0) ? __ldg(p.lse_gather + orow) : -1;
 #pragma unroll 1
     for (int cs = c0; cs < c1; cs += 128) {
@@ -320,8 +323,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
         const int n0 = n0_tile + c;
         if (n0 >= p.N) break;
         uint32_t acc[32];
-        tmem_ld_32x32(taddr + c, acc);
-        tmem_ld_wait();
+        acc_ld32<BN>(accs, arow, c, acc);
         float x[32];
         float cm = -INFINITY;
         if (n0 + 32 <= p.N && p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) {
@@ -379,6 +381,10 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       if (orow >= 0 && n0_tile + cs < ((p.N + 255) / 256) * 256)
         p.lse_part[(size_t)orow * p.lse_nslab + ((n0_tile + cs) >> 7)] = make_float2(m, ssum);
     }
+    // the last column tile also fills the slabs past the end of N (lse_slabs rounds up to 256 columns)
+    if (orow >= 0 && c1 > c0 && n0_tile + c1 >= p.N)
+      for (int sl = (n0_tile + c1) >> 7; sl < p.lse_nslab; ++sl)
+        p.lse_part[(size_t)orow * p.lse_nslab + sl] = make_float2(-INFINITY, 0.f);
   } else if constexpr (EPI == EPI_GLU) {
     if (p.glu_coalesced && ((c1 - c0) & 127) == 0) {
       // 128 accumulator columns = 64 outputs = 128 bytes per row per round through the staging tile (as for bf16)
@@ -391,8 +397,6 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       }
       bf16* out = reinterpret_cast<bf16*>(p.out);
       uint32_t* stage_u = reinterpret_cast<uint32_t*>(stage);
-      mbar_wait(tfull_bar, aphase);
-      tc_fence_after();
 #pragma unroll 1
       for (int c = c0; c < c1; c += 128) {
         if (n0_tile + c >= p.N) break;
@@ -403,9 +407,8 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
 #pragma unroll 1
         for (int hf = 0; hf < 2; ++hf) {  // two groups of 32 value + 32 gate columns -> 16-byte slots 4*hf .. 4*hf+3
           uint32_t av[32], gv[32];
-          tmem_ld_32x32(taddr + c + 64 * hf, av);
-          tmem_ld_32x32(taddr + c + 64 * hf + 32, gv);
-          tmem_ld_wait();
+          acc_ld32<BN>(accs, arow, c + 64 * hf, av);
+          acc_ld32<BN>(accs, arow, c + 64 * hf + 32, gv);
           const int n0 = n0_tile + c + 64 * hf;
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
@@ -458,15 +461,12 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       }
       return;
     }
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
 #pragma unroll 1
     for (int c = c0; c < c1; c += 64) {
       if (n0_tile + c >= p.N) break;
       uint32_t av[32], gv[32];
-      tmem_ld_32x32(taddr + c, av);
-      tmem_ld_32x32(taddr + c + 32, gv);
-      tmem_ld_wait();
+      acc_ld32<BN>(accs, arow, c, av);
+      acc_ld32<BN>(accs, arow, c + 32, gv);
       if (orow >= 0) store_glu(p, orow, n0_tile + c, av, gv);
     }
   } else if ((EPI == EPI_BF16 || EPI == EPI_BF16_RELU || EPI == EPI_BF16_SILU || EPI == EPI_BF16_RELPOS) &&
@@ -482,21 +482,18 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
     }
     bf16* out = reinterpret_cast<bf16*>(p.out);
     uint32_t* stage_u = reinterpret_cast<uint32_t*>(stage);
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
 #pragma unroll 1
     for (int c = c0; c < c1; c += 64) {
       if (n0_tile + c >= p.N) break;
       if (n0_tile + c + 64 <= p.N) {
         uint32_t acc[64];
-        tmem_ld_32x32(taddr + c, acc);
-        tmem_ld_32x32(taddr + c + 32, acc + 32);
-        tmem_ld_wait();
+        acc_ld32<BN>(accs, arow, c, acc);
+        acc_ld32<BN>(accs, arow, c + 32, acc + 32);
         const int n0 = n0_tile + c;
         // EPI_BF16_RELPOS: this 64-column chunk is one head of the KEY block -> K'' = k + pos[t], key bias u.k + vp
         bool kcols = false;
         int rp_t = 0, rp_hc = 0;
-        float rp_acc = 0.f;
+        float rp_part[8];   // u . k + v . pos over each 8-column slot, summed like relpos_prep_vec_kernel<8>
         if constexpr (EPI == EPI_BF16_RELPOS) {
           kcols = n0 >= p.rp_col0 && n0 < p.rp_col0 + p.rp_H * 64;
           rp_hc = n0 - p.rp_col0;
@@ -543,21 +540,27 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
               const float4 u0 = __ldg(reinterpret_cast<const float4*>(p.rp_u + rp_hc + 8 * j));
               const float4 u1 = __ldg(reinterpret_cast<const float4*>(p.rp_u + rp_hc + 8 * j) + 1);
               const float uu[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+              const float4 v0 = __ldg(reinterpret_cast<const float4*>(p.rp_v + rp_hc + 8 * j));
+              const float4 v1 = __ldg(reinterpret_cast<const float4*>(p.rp_v + rp_hc + 8 * j) + 1);
               const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z), p3 = unpack_bf16x2(pv.w);
               const float pp[8] = {p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x, p3.y};
+              float kq[8];
 #pragma unroll
               for (int e = 0; e < 8; ++e) {
-                const float kq = __bfloat162float(__float2bfloat16(v[e]));   // the key as the projection would store it
-                rp_acc = fmaf(uu[e], kq, rp_acc);
-                v[e] = kq + pp[e];
+                kq[e] = __bfloat162float(__float2bfloat16(v[e]));   // the key as the projection would store it
+                v[e] = kq[e] + pp[e];
               }
+              // the same expression as the separate kernel, so that both paths give the same bias bit for bit
+              rp_part[j] = uu[0] * kq[0] + uu[1] * kq[1] + uu[2] * kq[2] + uu[3] * kq[3] + uu[4] * kq[4] + uu[5] * kq[5] +
+                           uu[6] * kq[6] + uu[7] * kq[7] + v0.x * pp[0] + v0.y * pp[1] + v0.z * pp[2] + v0.w * pp[3] +
+                           v1.x * pp[4] + v1.y * pp[5] + v1.z * pp[6] + v1.w * pp[7];
             }
           }
           if (PAIR && part == 1) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) v[e] -= __bfloat162float(__float2bfloat16(v[e]));
           }
-          if (p.debug_skip_epi == 3 && v[0] != 123.456f) continue;  // tuning aid: TMEM loads + math only
+          if (p.debug_skip_epi == 3 && v[0] != 123.456f) continue;  // tuning aid: accumulator reads + math only
           *reinterpret_cast<uint4*>(stage_u + lane * 32 + ((j ^ (lane & 7)) << 2)) =
               make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
                          pack_bf16x2(v[6], v[7]));
@@ -576,15 +579,16 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
         if constexpr (EPI == EPI_BF16_RELPOS) {
           if (kcols && orow >= 0) {
             const int hh = rp_hc >> 6;
-            p.rp_cb[((orow / p.rp_T) * p.rp_H + hh) * (long long)p.rp_T + rp_t] = rp_acc + __ldg(p.rp_vp + (long long)hh * p.rp_T + rp_t);
+            // the separate kernel's shuffle reduction over the head's 8 lanes (xor 4, 2, 1)
+            p.rp_cb[((orow / p.rp_T) * p.rp_H + hh) * (long long)p.rp_T + rp_t] =
+                ((rp_part[0] + rp_part[4]) + (rp_part[2] + rp_part[6])) + ((rp_part[1] + rp_part[5]) + (rp_part[3] + rp_part[7]));
           }
         }
       } else {
         for (int cc = c; cc < c + 64 && cc < c1; cc += 32) {
           if (n0_tile + cc >= p.N) break;
           uint32_t acc[32];
-          tmem_ld_32x32(taddr + cc, acc);
-          tmem_ld_wait();
+          acc_ld32<BN>(accs, arow, cc, acc);
           if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + cc, acc);
         }
       }
@@ -604,13 +608,11 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       for (int it = 0; it < 8; ++it)
         if (ro[it] >= 0) r[it] = *reinterpret_cast<const float4*>(out + ro[it] + c0);
     }
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
 #pragma unroll 1
     for (int c = c0; c < c1; c += 32) {
       if (n0_tile + c >= p.N) break;
       uint32_t acc[32];
-      tmem_ld_32x32(taddr + c, acc);
+      acc_ld32<BN>(accs, arow, c, acc);
       const int n = n0_tile + c + slot * 4;       // first of this lane's 4 columns
       const bool vec = (n + 4 <= p.N);
       float4 rn[8];
@@ -630,7 +632,6 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
           if (n + 2 < p.N) b4.z = __ldg(p.bias + n + 2);
         }
       }
-      tmem_ld_wait();
 #pragma unroll
       for (int j = 0; j < 8; ++j)
         *reinterpret_cast<uint4*>(stage + lane * 32 + ((j ^ (lane & 7)) << 2)) =
@@ -664,52 +665,52 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       }
     }
   } else {
-    mbar_wait(tfull_bar, aphase);
-    tc_fence_after();
 #pragma unroll 1
     for (int c = c0; c < c1; c += 32) {
       if (n0_tile + c >= p.N) break;
       uint32_t acc[32];
-      tmem_ld_32x32(taddr + c, acc);
-      tmem_ld_wait();
+      acc_ld32<BN>(accs, arow, c, acc);
       if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + c, acc);
     }
   }
 }
 
-// warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2..9: epilogue (two warps per TMEM lane quarter, each
-// draining one half of the accumulator columns, so twice the loads / stores are in flight per tile)
-constexpr int kEpiWarps = 8;
-constexpr int kGemmThreads = 64 + 32 * kEpiWarps;
+// warps 0..7: two consumer warpgroups (wgmma on 64 rows each, then the epilogue of those rows), warp 8: TMA producer
+constexpr int kConsumerWGs = 2;
+constexpr int kGemmThreads = 128 * kConsumerWGs + 32;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
+  static constexpr int STAGES = 4;
   static constexpr uint32_t A_BYTES = BM * BK * 2;
   static constexpr uint32_t B_BYTES = BN * BK * 2;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + kEpiWarps * 4096 /*epilogue staging*/;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;
+  static constexpr uint32_t ACC_BYTES = BM * BN * 4;   // fp32 accumulator tile (epilogue copy)
+  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 8 * 4096 /*epilogue staging*/ + 256 /*barriers*/ +
+                                         1024 /*align slack*/;
 };
 
+// Persistent, warp-specialised TMA + wgmma GEMM (1 CTA / SM, grid = min(#tiles, #SMs), static round-robin tiles of
+// 128 x BN).  The producer fills a STAGES-deep ring of {A 128x64, W BNx64} bf16 tiles (SWIZZLE_128B).  Consumer
+// warpgroup g multiplies rows [64g, 64g+64) of every stage with 4 x wgmma m64nBNk16, releasing the previous stage as
+// soon as its MMAs have retired, then copies its accumulator to shared memory and drains it through the fused epilogue
+// (drain_tile) while the producer already streams the next tile's first stages.
 template <int BN, int EPI, bool PAIR>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const GemmKParams p) {
+gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  float* accs = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+  float* stage_epi = accs + Cfg::BM * BN;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_epi + 8 * 1024);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -717,280 +718,106 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], p.epi_warps);
+      mbar_init(&empty[i], 4 * kConsumerWGs);   // lane 0 of every consumer warp
     }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int nkb = p.num_k_blocks;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 * kConsumerWGs) {
     // ------------------------------------------------------------ TMA producer
-    uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      TileCoord t = decode_tile(p, tile, BN);
-      for (int kbx = 0; kbx < nkb; ++kbx) {
-        // bf16x3: pass 0 = A_hi W_hi, pass 1 = A_lo W_hi, pass 2 = A_hi W_lo
-        const int seg = p.x3 ? kbx / p.kb_seg : 0;
-        const int kb = kbx - seg * p.kb_seg;
-        const int a_ofs = (seg == 1) ? p.a_lo_ofs : 0, w_ofs = (seg == 2) ? p.w_lo_ofs : 0;
-        mbar_wait(&empty[stage], phase ^ 1);
-        mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-        if (p.conv_mode) {
-          int tap = kb / p.conv_cblocks;
-          int cb = kb - tap * p.conv_cblocks;
-          int kh = tap / 3, kw = tap - kh * 3;
-          tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], cb * 64 + a_ofs, 2 * t.f + kw, t.row0 + (kh >> 1),
-                      t.b * 2 + (kh & 1));
-        } else {
-          tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kb * 64 + a_ofs, t.row0, 0, 0);
-        }
-        tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kb * 64 + w_ofs, t.n0);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+    if (lane == 0) {
+      uint32_t stage = 0, phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        TileCoord t = decode_tile(p, tile, BN);
+        for (int kbx = 0; kbx < nkb; ++kbx) {
+          // bf16x3: pass 0 = A_hi W_hi, pass 1 = A_lo W_hi, pass 2 = A_hi W_lo
+          const int seg = p.x3 ? kbx / p.kb_seg : 0;
+          const int kb = kbx - seg * p.kb_seg;
+          const int a_ofs = (seg == 1) ? p.a_lo_ofs : 0, w_ofs = (seg == 2) ? p.w_lo_ofs : 0;
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+          if (p.conv_mode) {
+            int tap = kb / p.conv_cblocks;
+            int cb = kb - tap * p.conv_cblocks;
+            int kh = tap / 3, kw = tap - kh * 3;
+            tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], cb * 64 + a_ofs, 2 * t.f + kw, t.row0 + (kh >> 1),
+                        t.b * 2 + (kh & 1));
+          } else {
+            tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kb * 64 + a_ofs, t.row0, 0, 0);
+          }
+          tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kb * 64 + w_ofs, t.n0);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------------------------------------ MMA issuer (single thread)
-    // instruction descriptor: D=f32, A=B=bf16, both K-major, N=BN, M=128
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-    uint32_t stage = 0, phase = 0, as = 0, aphase = 0;
+  } else {
+    // ------------------------------------------------------------ consumer warpgroups
+    const int wg = warp >> 2, wl = warp & 3;
+    const int q = 2 * wg + (wl & 1);   // 32-row quarter of the tile this warp drains
+    const int chalf = wl >> 1;         // which half of the accumulator columns
+    // LSE partials and the coalesced GLU path work on 128-column slabs and the bf16 path on 64-column chunks: there (and
+    // for 64-wide tiles) one warp per row quarter takes all columns
+    constexpr bool whole = (EPI == EPI_LSE || EPI == EPI_GLU || BN == 64);
+    const int c0 = whole ? (chalf ? BN : 0) : chalf * (BN / 2);
+    const int c1 = whole ? BN : c0 + BN / 2;
+    float* stage_w = stage_epi + warp * 1024;
+    uint32_t stage = 0, phase = 0;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
+      TileCoord t = decode_tile(p, tile, BN);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(sA + stage * Cfg::A_BYTES));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(sB + stage * Cfg::B_BYTES));
+        const uint64_t adesc = make_sw128_desc(smem_u32(sA + stage * Cfg::A_BYTES + wg * (Cfg::A_BYTES / 2)));
+        const uint64_t bdesc = make_sw128_desc(smem_u32(sB + stage * Cfg::B_BYTES));
+        wgmma_fence_regs<BN / 2>(acc);
+        wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           // advance 16 bf16 = 32 B along K inside the 128 B swizzle span: +2 in the (addr >> 4) field
-          umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
+          if constexpr (BN == 128) wgmma_m64n128k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+          else wgmma_m64n64k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
         }
-        umma_commit(&empty[stage]);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous stage's MMAs have retired: hand its buffers back to the producer
+        wgmma_fence_regs<BN / 2>(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = (int)stage;
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      umma_commit(&tfull[as]);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-  } else if (warp >= 2 && warp < 2 + p.epi_warps) {
-    // ------------------------------------------------------------ epilogue warps
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int chalf = (warp - 2) >> 2;  // which half of the accumulator columns this warp drains
-    const int ccols = (p.epi_warps == 8) ? BN / 2 : BN;
-    float* stage = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256) + (warp - 2) * 1024;
-    uint32_t as = 0, aphase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      TileCoord t = decode_tile(p, tile, BN);
-      drain_tile<EPI, PAIR>(p, t, q, lane, tmem_base + ((uint32_t)(q * 32) << 16) + as * BN, chalf * ccols,
-                      (chalf + 1) * ccols, &tfull[as], aphase, stage);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 2-CTA variant (cta_group::2): a CTA pair (cluster 2x1x1, same TPC) owns a 256 x BN tile.  Each CTA stages its own
-// 128 A rows and HALF of the B rows per k-block (32 KB / stage / SM instead of 48 KB), the leader CTA issues
-// tcgen05.mma.cta_group::2 (M = 256) which reads both CTAs' shared memory and writes both CTAs' TMEM; TMA transaction
-// bytes of both CTAs are credited to the leader's `full` barrier, tcgen05.commit multicasts the `empty` / `tmem full`
-// arrivals to both CTAs, and both CTAs' epilogue warps arrive on the leader's `tmem empty` barrier.
-template <int BN>
-struct Gemm2Cfg {
-  static constexpr int BK = 64;
-  static constexpr uint32_t A_BYTES = 128 * BK * 2;
-  static constexpr uint32_t B_BYTES = (BN / 2) * BK * 2;
-  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 6 : 8;
-  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + kEpiWarps * 4096;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;
-};
-
-template <int BN, int EPI, bool PAIR>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const GemmKParams p) {
-  using Cfg = Gemm2Cfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = (rank == 0);
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);   // the leader's producer arrives with the byte count of BOTH CTAs' loads
-      mbar_init(&empty[i], 1);  // multicast tcgen05.commit
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 2 * p.epi_warps);  // epilogue warps of both CTAs (on the leader's copy)
-    }
-    fence_barrier_init();
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
-    tmem_alloc_2sm(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish_2sm();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int nkb = p.num_k_blocks;
-
-  auto tile_coord = [&](int tile) {
-    // cluster tile: 256 rows; this CTA owns rows [rank*128, rank*128+128) of it
-    TileCoord t;
-    int nb = tile % p.tiles_n;
-    int mt = tile / p.tiles_n;
-    t.n0 = nb * BN;
-    if (p.conv_mode) {
-      t.f = mt % p.conv_F2;
-      int r = mt / p.conv_F2;
-      t.row0 = (r % p.conv_tt) * 256 + (int)rank * 128;
-      t.b = r / p.conv_tt;
-    } else {
-      t.row0 = mt * 256 + (int)rank * 128;
-      t.b = 0;
-      t.f = 0;
-    }
-    return t;
-  };
-
-  if (warp == 0 && lane == 0) {
-    // ------------------------------------------------------------ TMA producer (both CTAs)
-    uint32_t stage = 0, phase = 0;
-    for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
-      TileCoord t = tile_coord(tile);
-      for (int kbx = 0; kbx < nkb; ++kbx) {
-        const int seg = p.x3 ? kbx / p.kb_seg : 0;   // bf16x3 passes, see gemm_tc_kernel
-        const int kb = kbx - seg * p.kb_seg;
-        const int a_ofs = (seg == 1) ? p.a_lo_ofs : 0, w_ofs = (seg == 2) ? p.w_lo_ofs : 0;
-        mbar_wait(&empty[stage], phase ^ 1);
-        // Only the leader arrives (expecting both CTAs' bytes).  The peer cannot run a phase ahead: its `empty`
-        // barrier is released by the leader's tcgen05.commit, i.e. after the leader consumed this phase.
-        if (leader) mbar_expect_tx(&full[stage], 2 * Cfg::STAGE_BYTES);
-        if (p.conv_mode) {
-          int tap = kb / p.conv_cblocks;
-          int cb = kb - tap * p.conv_cblocks;
-          int kh = tap / 3, kw = tap - kh * 3;
-          tma_load_4d_2sm(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], cb * 64 + a_ofs, 2 * t.f + kw,
-                          t.row0 + (kh >> 1), t.b * 2 + (kh & 1));
-        } else {
-          tma_load_4d_2sm(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kb * 64 + a_ofs, t.row0, 0, 0);
-        }
-        tma_load_2d_2sm(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kb * 64 + w_ofs, t.n0 + (int)rank * (BN / 2));
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && lane == 0 && leader) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA, single thread)
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((256u >> 4) << 24);
-    uint32_t stage = 0, phase = 0, as = 0, aphase = 0;
-    for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
-      mbar_wait(&tempty[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(sA + stage * Cfg::A_BYTES));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(sB + stage * Cfg::B_BYTES));
+      wgmma_wait<0>();
+      wgmma_fence_regs<BN / 2>(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      // accumulator -> shared memory (this warpgroup's 64 rows; the previous tile's drain of them is finished)
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      {
+        const int r0 = wg * 64 + wl * 16 + (lane >> 2);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-        umma_commit_2sm(&empty[stage], 3);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int r = r0 + 8 * i;
+            *reinterpret_cast<float2*>(accs + r * BN + ((((c >> 2)) ^ (r & 7)) << 2) + (c & 3)) =
+                make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+          }
         }
       }
-      umma_commit_2sm(&tfull[as], 3);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      drain_tile<BN, EPI, PAIR>(p, t, q, lane, accs, c0, c1, stage_w);
     }
-  } else if (warp >= 2 && warp < 2 + p.epi_warps) {
-    // ------------------------------------------------------------ epilogue warps (both CTAs, own 128 rows)
-    const int q = warp & 3;
-    const int chalf = (warp - 2) >> 2;
-    const int ccols = (p.epi_warps == 8) ? BN / 2 : BN;
-    float* stage = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256) + (warp - 2) * 1024;
-    uint32_t as = 0, aphase = 0;
-    for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
-      TileCoord t = tile_coord(tile);
-      drain_tile<EPI, PAIR>(p, t, q, lane, tmem_base + ((uint32_t)(q * 32) << 16) + as * BN, chalf * ccols,
-                      (chalf + 1) * ccols, &tfull[as], aphase, stage);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tempty[as]);
-        else mbar_arrive_remote(&tempty[as], 0);
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
@@ -1130,9 +957,8 @@ struct GemmProfRec {
 static bool g_prof_on = false;
 static std::vector<GemmProfRec> g_prof;
 static std::mutex g_prof_mutex;
-// Events are pooled per device and reused across profiling windows: creating two per launch inside the timed region cost
-// host time exactly where the step is host-sensitive (two ranks on one node: the device-resident run measured slower than
-// the end-to-end run that follows it without profiling).
+// Events are pooled per device and reused across profiling windows: creating two per launch inside the timed region
+// would cost host time exactly where the step is host-sensitive.
 constexpr int kProfMaxDev = 64;
 static std::vector<cudaEvent_t> g_prof_pool[kProfMaxDev];
 static size_t g_prof_pool_used[kProfMaxDev];
@@ -1176,7 +1002,7 @@ int gemm_profile_end(double* total_ms, double* total_flops, long long* launches)
 }
 
 template <int BN>
-static int launch_tc(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
+static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   CUtensorMap tmA, tmB;
   const int kmul = a.x3 ? 2 : 1;
@@ -1202,15 +1028,15 @@ static int launch_tc(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
   void (*kern)(const CUtensorMap, const CUtensorMap, const GemmKParams) = nullptr;
   const bool pair = a.out_split > 0;
   switch (a.rp_pos ? (int)EPI_BF16_RELPOS : select_epi(a.act, a.out_mode)) {
-    case EPI_BF16: kern = pair ? gemm_tc_kernel<BN, EPI_BF16, true> : gemm_tc_kernel<BN, EPI_BF16, false>; break;
-    case EPI_BF16_RELU: kern = pair ? gemm_tc_kernel<BN, EPI_BF16_RELU, true> : gemm_tc_kernel<BN, EPI_BF16_RELU, false>; break;
-    case EPI_BF16_SILU: kern = pair ? gemm_tc_kernel<BN, EPI_BF16_SILU, true> : gemm_tc_kernel<BN, EPI_BF16_SILU, false>; break;
-    case EPI_F32: kern = gemm_tc_kernel<BN, EPI_F32, false>; break;
-    case EPI_RESID: kern = gemm_tc_kernel<BN, EPI_RESID, false>; break;
-    case EPI_GLU: kern = pair ? gemm_tc_kernel<BN, EPI_GLU, true> : gemm_tc_kernel<BN, EPI_GLU, false>; break;
-    case EPI_LSE: kern = gemm_tc_kernel<BN, EPI_LSE, false>; break;
-    case EPI_BF16_RELPOS: kern = gemm_tc_kernel<BN, EPI_BF16_RELPOS, false>; break;
-    default: kern = gemm_tc_kernel<BN, EPI_GENERIC, false>; break;
+    case EPI_BF16: kern = pair ? gemm_wg_kernel<BN, EPI_BF16, true> : gemm_wg_kernel<BN, EPI_BF16, false>; break;
+    case EPI_BF16_RELU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_RELU, true> : gemm_wg_kernel<BN, EPI_BF16_RELU, false>; break;
+    case EPI_BF16_SILU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_SILU, true> : gemm_wg_kernel<BN, EPI_BF16_SILU, false>; break;
+    case EPI_F32: kern = gemm_wg_kernel<BN, EPI_F32, false>; break;
+    case EPI_RESID: kern = gemm_wg_kernel<BN, EPI_RESID, false>; break;
+    case EPI_GLU: kern = pair ? gemm_wg_kernel<BN, EPI_GLU, true> : gemm_wg_kernel<BN, EPI_GLU, false>; break;
+    case EPI_LSE: kern = gemm_wg_kernel<BN, EPI_LSE, false>; break;
+    case EPI_BF16_RELPOS: kern = gemm_wg_kernel<BN, EPI_BF16_RELPOS, false>; break;
+    default: kern = gemm_wg_kernel<BN, EPI_GENERIC, false>; break;
   }
   RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES));
   p.tiles_n = (a.N + BN - 1) / BN;
@@ -1224,69 +1050,6 @@ static int launch_tc(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
     RVB_CHECK_CUDA(cudaEventRecord(rec.a, stream));
   }
   kern<<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  RVB_COUNT_LAUNCH();
-  RVB_CHECK_LAUNCH();
-  if (g_prof_on) {
-    RVB_CHECK_CUDA(cudaEventRecord(rec.b, stream));
-    {
-      std::lock_guard<std::mutex> lock(g_prof_mutex);
-      g_prof.push_back(rec);
-    }
-  }
-  return 0;
-}
-
-template <int BN>
-static int launch_tc2(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BN>;
-  CUtensorMap tmA, tmB;
-  const int kmul = a.x3 ? 2 : 1;
-  const long long lda = a.lda ? a.lda : (long long)a.K * kmul, ldw = a.ldw ? a.ldw : (long long)a.K * kmul;
-  if (a.conv_mode) {
-    const cuuint64_t Cp = (cuuint64_t)a.conv_C * (a.x3 ? 2 : 1);  // physical channels: [hi C | lo C] in bf16x3 mode
-    cuuint64_t dims[4] = {Cp, (cuuint64_t)a.conv_F1, (cuuint64_t)a.conv_T1h, (cuuint64_t)(2 * a.conv_B)};
-    cuuint64_t str[3] = {Cp * 2, (cuuint64_t)a.conv_F1 * Cp * 2, (cuuint64_t)a.conv_T1h * a.conv_F1 * Cp * 2};
-    cuuint32_t box[4] = {64, 1, 128, 1};
-    if (make_tmap(&tmA, a.A, 4, dims, str, box)) return -1;
-  } else {
-    cuuint64_t dims[4] = {(cuuint64_t)a.K * (a.x3 ? 2 : 1), (cuuint64_t)a.M, 1, 1};
-    cuuint64_t str[3] = {(cuuint64_t)lda * 2, (cuuint64_t)lda * 2 * a.M, (cuuint64_t)lda * 2 * a.M};
-    cuuint32_t box[4] = {64, 128, 1, 1};
-    if (make_tmap(&tmA, a.A, 4, dims, str, box)) return -1;
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)a.K * (a.x3 ? 2 : 1), (cuuint64_t)a.N};
-    cuuint64_t str[1] = {(cuuint64_t)ldw * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)(BN / 2)};
-    if (make_tmap(&tmB, a.W, 2, dims, str, box)) return -1;
-  }
-  void (*kern)(const CUtensorMap, const CUtensorMap, const GemmKParams) = nullptr;
-  const bool pair = a.out_split > 0;
-  switch (a.rp_pos ? (int)EPI_BF16_RELPOS : select_epi(a.act, a.out_mode)) {
-    case EPI_BF16: kern = pair ? gemm_tc2_kernel<BN, EPI_BF16, true> : gemm_tc2_kernel<BN, EPI_BF16, false>; break;
-    case EPI_BF16_RELU: kern = pair ? gemm_tc2_kernel<BN, EPI_BF16_RELU, true> : gemm_tc2_kernel<BN, EPI_BF16_RELU, false>; break;
-    case EPI_BF16_SILU: kern = pair ? gemm_tc2_kernel<BN, EPI_BF16_SILU, true> : gemm_tc2_kernel<BN, EPI_BF16_SILU, false>; break;
-    case EPI_F32: kern = gemm_tc2_kernel<BN, EPI_F32, false>; break;
-    case EPI_RESID: kern = gemm_tc2_kernel<BN, EPI_RESID, false>; break;
-    case EPI_GLU: kern = pair ? gemm_tc2_kernel<BN, EPI_GLU, true> : gemm_tc2_kernel<BN, EPI_GLU, false>; break;
-    case EPI_LSE: kern = gemm_tc2_kernel<BN, EPI_LSE, false>; break;
-    case EPI_BF16_RELPOS: kern = gemm_tc2_kernel<BN, EPI_BF16_RELPOS, false>; break;
-    default: kern = gemm_tc2_kernel<BN, EPI_GENERIC, false>; break;
-  }
-  RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES));
-  p.tiles_n = (a.N + BN - 1) / BN;
-  if (a.conv_mode) p.conv_tt = (a.conv_T2 + 255) / 256;
-  int tiles_m = a.conv_mode ? a.conv_B * a.conv_F2 * p.conv_tt : (a.M + 255) / 256;
-  p.num_tiles = tiles_m * p.tiles_n;
-  int clusters = g_num_sms / 2;
-  if (p.num_tiles < clusters) clusters = p.num_tiles;
-  GemmProfRec rec;
-  if (g_prof_on) {
-    if (prof_event(&rec.a) || prof_event(&rec.b)) return -1;
-    rec.flops = 2.0 * (double)a.M * (double)a.N * (double)a.K * (a.x3 ? 3.0 : 1.0);
-    RVB_CHECK_CUDA(cudaEventRecord(rec.a, stream));
-  }
-  kern<<<2 * clusters, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
   if (g_prof_on) {
@@ -1344,12 +1107,13 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   p.rp_H = a.rp_H;
   p.rp_col0 = a.rp_col0;
   p.rp_u = a.rp_u;
-  p.rp_vp = a.rp_vp;
+  p.rp_v = a.rp_v;
   p.rp_cb = a.rp_cb;
   if (a.rp_pos) {
     RVB_REQUIRE(a.out_mode == OUT_BF16 && a.act == ACT_NONE && a.out_split == 0 && !a.conv_mode && a.rp_T > 0 &&
-                    a.rp_col0 % 64 == 0 && a.rp_ldp % 8 == 0 && a.N % 64 == 0 && a.rp_u && a.rp_vp && a.rp_cb &&
-                    (reinterpret_cast<uintptr_t>(a.rp_pos) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.rp_u) & 15) == 0,
+                    a.rp_col0 % 64 == 0 && a.rp_ldp % 8 == 0 && a.N % 64 == 0 && a.rp_u && a.rp_v && a.rp_cb &&
+                    (reinterpret_cast<uintptr_t>(a.rp_pos) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.rp_u) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(a.rp_v) & 15) == 0,
                 "gemm: rel-pos epilogue needs a plain bf16 output, 64-aligned key columns and 16-byte aligned tables");
     RVB_REQUIRE(get_gemm_impl() != 1, "gemm: rel-pos epilogue is not built for the simt bring-up kernel");
   }
@@ -1359,12 +1123,6 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     RVB_REQUIRE(get_gemm_impl() != 1, "gemm: OUT_LSE is not built for the simt bring-up kernel");
   }
   {
-    static int forced = -1;  // RVB_GEMM_EPI_WARPS=4|8 overrides the K-based choice (tuning aid)
-    if (forced < 0) {
-      const char* e = getenv("RVB_GEMM_EPI_WARPS");
-      forced = (e && (atoi(e) == 4 || atoi(e) == 8)) ? atoi(e) : 0;
-    }
-    p.epi_warps = forced ? forced : ((a.K <= 2048) ? 8 : 4);
     static int skip = -1;
     if (skip < 0) {
       const char* e = getenv("RVB_GEMM_SKIP_EPI");
@@ -1407,7 +1165,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     p.tiles_n = ((a.act == ACT_GLU ? a.N / 2 : a.N) + 31) / 32;
     int tiles_m = a.conv_mode ? a.conv_B * a.conv_F2 * p.conv_tt : (a.M + 127) / 128;
     p.num_tiles = tiles_m * p.tiles_n;
-    int grid = p.num_tiles < 148 * 8 ? p.num_tiles : 148 * 8;
+    int grid = p.num_tiles < g_num_sms * 8 ? p.num_tiles : g_num_sms * 8;
     gemm_simt_kernel<<<grid, 256, 0, stream>>>(p);
     RVB_COUNT_LAUNCH();
     RVB_CHECK_LAUNCH();
@@ -1417,12 +1175,11 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
               "gemm: operands must be 16-byte aligned");
   RVB_REQUIRE((p.lda * 2) % 16 == 0 && (p.ldw * 2) % 16 == 0, "gemm: leading dimensions must be multiples of 8");
   if (get_encode_fn()) return -1;
-  if (get_gemm_impl() == 2) {
-    if (a.N > 128) return launch_tc2<256>(a, p, stream);
-    return launch_tc2<128>(a, p, stream);
-  }
-  if (a.N > 128) return launch_tc<256>(a, p, stream);
-  return launch_tc<128>(a, p, stream);
+  // 64-wide tiles for narrow outputs; RVB_GEMM=narrow (impl 2) takes them for every shape whose epilogue allows it:
+  // all but the log-sum-exp partials (128-column slabs) and GLU hi/lo pairs (written 128 accumulator columns at a time)
+  const bool narrow = a.N <= 64 || (get_gemm_impl() == 2 && a.out_mode != OUT_LSE && !(a.act == ACT_GLU && a.out_split > 0));
+  if (!narrow) return launch_wg<128>(a, p, stream);
+  return launch_wg<64>(a, p, stream);
 }
 
 }  // namespace rvb

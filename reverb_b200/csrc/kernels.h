@@ -1,4 +1,4 @@
-// reverb_b200 — host-side launchers of the sm_100a kernels (internal; the public boundary is
+// reverb_b200 — host-side launchers of the sm_90a kernels (internal; the public boundary is
 // include/rvb_b200.h).  Every launcher enqueues on the given stream and returns 0 / <0.
 #pragma once
 #include "common.cuh"
@@ -57,13 +57,14 @@ struct GemmArgs {
   int conv_pair_out = 0;
   // rel-pos attention folded into the fused [q; k; v] projection (OUT_BF16, no activation, d_k = 64): the epilogue
   // replaces the key columns [rp_col0, rp_col0 + rp_H*64) by K'' = bf16(k + pos[t]) (t = row % rp_T, pos row stride
-  // rp_ldp) and writes the per-key bias rp_cb[(row / rp_T) * rp_H + h, t] = u_h . k + rp_vp[h, t] — what the separate
-  // relpos_prep kernel (attention_tc.cu) computes from the stored projection; rp_vp[h, t] = v_h . pos[t, h] is
-  // input-independent (launch_relpos_vp).
+  // rp_ldp) and writes the per-key bias rp_cb[(row / rp_T) * rp_H + h, t] = u_h . k + v_h . pos[t] — what the separate
+  // relpos_prep kernel (attention_tc.cu) computes from the stored projection, in the same summation order, so that the
+  // fused and the separate path give the same bias bit for bit (a precomputed v . pos table rounds differently, and the
+  // encoder layers amplify that difference).  v . pos costs 8 FMAs per key column here, next to the pos load.
   const bf16* rp_pos = nullptr;
   int rp_ldp = 0, rp_T = 0, rp_H = 0, rp_col0 = 0;
   const float* rp_u = nullptr;
-  const float* rp_vp = nullptr;
+  const float* rp_v = nullptr;
   float* rp_cb = nullptr;
   // OUT_LSE
   const int* lse_gather = nullptr;   // (M) column index per row, < 0 = none
@@ -75,10 +76,10 @@ int launch_lse_merge(const float2* part, int slabs, const float* tgt, const int*
                      cudaStream_t stream);
 
 int launch_gemm(const GemmArgs& a, cudaStream_t stream);
-// 0 = tcgen05/TMA kernel (default), 1 = plain CUDA-core debug kernel (env RVB_GEMM=simt)
+// 0 = wgmma/TMA kernel (default), 1 = plain CUDA-core debug kernel (env RVB_GEMM=simt), 2 = wgmma with 64-wide tiles
 void set_gemm_impl(int impl);
 int get_gemm_impl();
-// per-launch CUDA-event timing of the tcgen05 GEMM (algorithmic FLOPs = 2*M*N*K per launch)
+// per-launch CUDA-event timing of the wgmma GEMM (algorithmic FLOPs = 2*M*N*K per launch)
 void gemm_profile_begin();
 int gemm_profile_end(double* total_ms, double* total_flops, long long* launches);
 
@@ -163,7 +164,7 @@ struct AttnArgs {
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 
-// tcgen05 attention (attention_tc.cu): d_k = 64, key-length mask, optional per-key bias (rel-pos folded, see the
+// wgmma attention (attention_tc.cu): d_k = 64, key-length mask, optional per-key bias (rel-pos folded, see the
 // kernel header).  Rows are grouped: group g owns query rows [g*Tq, (g+1)*Tq) and key rows [g*Tk, (g+1)*Tk);
 // the q/k/v pointers address column 0 of head 0 (heads are 64 columns apart).
 struct AttnTcArgs {
@@ -184,9 +185,6 @@ struct AttnTcArgs {
   float scale = 1.0f;
 };
 int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream);
-// vp[l, h, t] = v_{l,h} . pos[t, l*d + h*dk ...]  (pos: (T, L*d) bf16 = all layers' linear_pos(pos_emb); bias_v: (L, d))
-int launch_relpos_vp(const bf16* pos, int ldp, const float* bias_v_all, float* vp, int T, int L, int H, int dk,
-                     cudaStream_t stream);
 // K'' = k + pos (bf16, (B*T, H*dk) dense) and cbias[b,h,t] = u_h . k + v_h . pos
 int launch_relpos_prep(const bf16* k, int ldk, const bf16* pos, int ldp, const float* bias_u, const float* bias_v,
                        bf16* kpp, float* cbias, int B, int T, int H, int dk, cudaStream_t stream);

@@ -1,7 +1,7 @@
 """WeSpeaker ResNet34 speaker-embedding model on the GPU (csrc/diar_emb.cu through include/rvb_diar.h).
 
 Mirror of what the reference obtains from `pyannote.audio` (`PyannoteAudioPretrainedSpeakerEmbedding.__call__(waveforms,
-masks)` inside `SpeakerDiarization.get_embeddings`, behind /root/reference/diarization/infer_pyannote3.0.py:33-40).
+masks)` inside `SpeakerDiarization.get_embeddings`, behind diarization/infer_pyannote3.0.py:33-40).
 ** parity unpinned **: see include/rvb_diar.h.  No CPU fallback.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """`python -m reverb_b200.diarization.infer AUDIO... --out-dir DIR [--pipeline-model DIR | --synthetic]`
 
-CLI mirror of /root/reference/diarization/infer_pyannote3.0.py:16-42 (positional audios, --out-dir, --pipeline-model,
+CLI mirror of diarization/infer_pyannote3.0.py:16-42 (positional audios, --out-dir, --pipeline-model,
 --hf-access-token; output `<out-dir>/<basename>.rttm`).  Differences forced by the environment: there is no network, so
 `--pipeline-model` names a LOCAL directory holding `segmentation.pt` and `embedding.pt` (torch state_dicts under
 pyannote's key names, what `Model.from_pretrained(...).state_dict()` saves for the pipeline's two models) and the

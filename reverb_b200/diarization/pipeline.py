@@ -1,6 +1,6 @@
 """Speaker-diarization pipeline around the two GPU networks (segmentation.py, embedding.py).
 
-What the reference runs (/root/reference/diarization/infer_pyannote3.0.py:33-42):
+What the reference runs (reference: diarization/infer_pyannote3.0.py:33-42):
 
     pipeline = Pipeline.from_pretrained('Revai/reverb-diarization-v1'); annotation = pipeline(audio)
     annotation.write_rttm(f)
@@ -87,7 +87,8 @@ def aggregate(scores: np.ndarray, chunks: SlidingWindow, frames: SlidingWindow, 
 
 def condensed_euclidean(emb: np.ndarray, device: Optional[str] = None) -> np.ndarray:
     """scipy `pdist(emb)` (float64, direct differences) computed with torch on `device`: for the ~8 000 embeddings of a
-    45-minute recording the pairwise distances are 70 % of the clustering time on the host and milliseconds on the GPU.
+    45-minute recording the pairwise distances are a large share of the clustering time on the host (not re-timed on the
+    H100).
     The linkage itself stays scipy's (same dendrogram: `linkage(y)` == `linkage(X)` for Euclidean input)."""
     x = torch.from_numpy(np.ascontiguousarray(emb, dtype=np.float64)).to(device or "cpu")
     n = x.shape[0]
@@ -212,8 +213,8 @@ class SpeakerDiarization:
         self.min_duration_off = min_duration_off
         self.exclude_overlap = embedding_exclude_overlap
         self.batch_size = batch_size
-        # the LSTM recurrence runs 8 windows per 2-CTA cluster and direction: 296 windows fill the 148 SMs of a B200
-        self.seg_batch_size = segmentation_batch_size or max(batch_size, 296)
+        # the LSTM recurrence runs 8 windows per 2-CTA cluster and direction: 264 windows fill the 132 SMs of an H100
+        self.seg_batch_size = segmentation_batch_size or max(batch_size, 264)
         self.embedding_min_samples = embedding_min_samples
         self.mapping = powerset_mapping(max_speakers_per_chunk, max_speakers_per_frame)
         self.frames = receptive_field(sample_rate)

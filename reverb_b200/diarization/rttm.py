@@ -2,7 +2,7 @@
 
 Reference: diarization/infer_pyannote3.0.py:40-42 (`annotation.write_rttm(f)`, pyannote.core.Annotation) and
 diarization/assign_words2speakers.py:75-81 (`pyannote.database.util.load_rttm` + `itertracks(yield_label=True)`).
-pyannote is a third-party dependency absent from /root/reference (diarization/requirements.txt:1 pins
+pyannote is a third-party dependency not vendored in the reference repository (diarization/requirements.txt:1 pins
 pyannote.audio==3.3.1); its published RTTM conventions are restated here:
 
     SPEAKER <uri> 1 <start:.3f> <duration:.3f> <NA> <NA> <label> <NA> <NA>

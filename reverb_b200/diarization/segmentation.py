@@ -1,7 +1,7 @@
 """PyanNet segmentation model on the GPU (csrc/diar_seg.cu through the C ABI of include/rvb_diar.h).
 
 Mirror of what the reference obtains from `pyannote.audio` (`Model` called on (batch, channel, sample) windows inside
-`SpeakerDiarization.get_segmentations`, behind /root/reference/diarization/infer_pyannote3.0.py:33-40), plus the
+`SpeakerDiarization.get_segmentations`, behind diarization/infer_pyannote3.0.py:33-40), plus the
 powerset -> multilabel conversion (`pyannote.audio.utils.powerset.Powerset.to_multilabel`).  ** parity unpinned **:
 see include/rvb_diar.h.  No CPU fallback: construction fails without the CUDA library / a CUDA device.
 """

@@ -1,6 +1,6 @@
 """Host-side handle of the native model plan (librvb_b200.so): PyTorch tensors in, PyTorch
 tensors / Python lists out.  PyTorch is used for device memory and streams only; every
-FLOP of the hot path runs in the hand-written sm_100a kernels behind the C ABI.
+FLOP of the hot path runs in the hand-written sm_90a kernels behind the C ABI.
 """
 from __future__ import annotations
 
@@ -38,7 +38,7 @@ PRECISIONS = {"bf16": 0, "fp32": 1, "bf16x3": 1}
 
 def resolve_precision(precision: Optional[str]) -> str:
     """'bf16' (default: bf16 tensor-core operands, fp32 accumulation — the throughput mode) or 'fp32' (= 'bf16x3': every
-    GEMM runs as three tcgen05 passes over (hi, lo) bf16 operand pairs and the attention in fp32 — reference-level
+    GEMM runs as three wgmma passes over (hi, lo) bf16 operand pairs and the attention in fp32 — reference-level
     accuracy at ~3x the tensor work).  None -> environment variable RVB_PRECISION, else 'bf16'."""
     import os
     p = precision if precision is not None else os.environ.get("RVB_PRECISION", "bf16")
@@ -94,7 +94,7 @@ class Engine:
     def __init__(self, configs: Dict, state_dict: Dict[str, torch.Tensor], vocab: int, device: torch.device,
                  precision: Optional[str] = None):
         if device.type != "cuda" or not torch.cuda.is_available():
-            raise RuntimeError("reverb_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("reverb_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.load()
         self.device = device
         self.precision = resolve_precision(precision)

@@ -1,6 +1,6 @@
 """`ReverbASR` / `load_model` — the public Python API, a drop-in for the reference's
 asr/wenet/cli/reverb.py (same class, method names, argument names, defaults and error
-behaviour), running on the native B200 engine.
+behaviour), running on the native H100 engine.
 
 Differences that are deliberate and documented in DESIGN.md:
   * the model always runs on a CUDA device (`gpu < 0` selects the current device; there
@@ -57,7 +57,7 @@ class ReverbASR:
                  precision: str | None = None):
         self.jit = False
         if not torch.cuda.is_available():
-            raise RuntimeError("reverb_b200.ReverbASR needs a CUDA device (B200, sm_100a); no CPU fallback exists")
+            raise RuntimeError("reverb_b200.ReverbASR needs a CUDA device (H100, sm_90a); no CPU fallback exists")
         self.device = torch.device("cuda", gpu if gpu >= 0 else torch.cuda.current_device())
         self.checkpoint = checkpoint
         with open(config, "r") as fin:
@@ -94,7 +94,7 @@ class ReverbASR:
             # no GlobalCMVN module in the reference model: the engine's fused (x - mean) * istd becomes the identity
             sd["encoder.global_cmvn.mean"] = torch.zeros(input_dim)
             sd["encoder.global_cmvn.istd"] = torch.ones(input_dim)
-        # precision: 'bf16' (default, throughput) or 'fp32' (bf16x3 tcgen05 passes + fp32 attention: reference-level
+        # precision: 'bf16' (default, throughput) or 'fp32' (bf16x3 wgmma passes + fp32 attention: reference-level
         # accuracy, engine.resolve_precision); None -> $RVB_PRECISION.  Not a reference argument: an extension.
         self.engine = Engine(self.configs, sd, self.configs["output_dim"], self.device, precision)
         self.model = ASRModel(self.engine, self.configs, self.configs["output_dim"])

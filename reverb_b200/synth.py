@@ -12,7 +12,7 @@ language-specific first/last blocks and an (LSL) bi-transformer decoder
 (SURVEY.md §8a quirk 9); `tests/test_oracle_vs_reference.py` checks this by a
 strict `load_state_dict` into the live reference model.
 
-This module does not depend on the reference and runs on the GPU box.
+This module does not depend on the reference; the GPU tests and the benchmark use it.
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ log-probs and accepted `> 98 %` / `0.5x-2x` / `>= 50 %` agreement.  Here the com
     (pinned bit-identical to the live reference, tests/test_oracle_vs_reference.py) on 2 x 30 s chunks.
 
 Any token-level exception is REPORTED (frame, margin) and bounded; bit-exactness of greedy ids is asserted.
-Measured values are printed (`pytest -s`) and collected in profiles/r2_parity.json by tools/parity_report.py.
+Measured values are printed (`pytest -s`); RVB_PARITY_LOG=<file> appends them as JSON lines.
 """
 import json
 import os
@@ -222,7 +222,7 @@ def test_beam_size_limit_is_reported_before_decoding(asr, model_dirs):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# fp32-accurate mode (precision="fp32": bf16x3 tcgen05 GEMMs + fp32 attention)
+# fp32-accurate mode (precision="fp32": bf16x3 wgmma GEMMs + fp32 attention)
 @pytest.fixture(scope="module")
 def asr_acc(model_dirs):
     import reverb_b200
@@ -231,10 +231,9 @@ def asr_acc(model_dirs):
 
 @pytest.mark.parametrize("case", ["causal_ln", "sym_bn"])
 def test_accurate_mode_matches_the_live_reference(asr_acc, golden_cases, case):
-    """precision='fp32' against the live reference's tensors and tokens (tests/golden): encoder_out rel-RMS < 2e-5
-    (measured 8e-6), CTC log-probs to 1e-3 abs (measured 1.5e-4; the reference's own precedent is rtol 1e-3 / atol 1e-5,
-    export_onnx_gpu.py:735-743), token confidences to 1e-3 (measured 1e-7), and EVERY token / n-best / time / pick
-    identical."""
+    """precision='fp32' against the live reference's tensors and tokens (tests/golden): encoder_out rel-RMS < 2e-5,
+    CTC log-probs to 1e-3 abs (the reference's own precedent is rtol 1e-3 / atol 1e-5, export_onnx_gpu.py:735-743),
+    token confidences to 1e-3, and EVERY token / n-best / time / pick identical."""
     meta, arr = golden_cases[case]
     m = asr_acc[case]
     assert m.engine.precision == "fp32"
@@ -327,8 +326,8 @@ def test_bench_shape_two_chunks_vs_oracle(bench_model_dir):
     """d=1024 / H=16 / L=18 / V=10001 / T'=748 (the ONLY shape BENCH / SCALE time), bf16 mode: fbank, encoder_out, CTC
     log-probs, greedy ids, prefix n-best and the rescoring pick of 2 x 30 s chunks vs the CPU oracle (fp32, the
     reference's ATen operators).  Stated tolerances (bf16 GEMM operands, fp32 accumulation, 18 blocks): encoder rel-RMS
-    < 1.2e-2 (measured 4.7e-3), log-prob |diff| < 0.25 on entries with p > e^-12 (measured 0.09); arg-max agreement
-    > 99 % with every exception a near-tie (measured: 3 of 1496 frames, oracle margins 0.003 - 0.018)."""
+    < 1.2e-2, log-prob |diff| < 0.25 on entries with p > e^-12; arg-max agreement > 99 % with every exception a
+    near-tie."""
     import reverb_b200
     from oracle import fbank_np, pipeline_ref
     from reverb_b200 import synth

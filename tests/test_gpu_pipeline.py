@@ -77,7 +77,7 @@ def test_fbank_and_encoder_vs_reference_fixture(asr, golden_cases, model_dirs, c
             n = int(enc_lens[b])
             # log-probs on the entries that matter (p > e^-12).  The synthetic CTC head is scaled x6
             # (logit sigma ~3.5, reverb_b200/synth.py), which amplifies the bf16 encoder error by the same factor:
-            # stated tolerance 0.12 abs (max over ~7k entries), 0.025 RMS (measured 0.06 / 0.015).
+            # stated tolerance 0.12 abs (max over ~7k entries), 0.025 RMS.
             sel = refp[b, :n] > -12
             diff = logp[b, :n][sel] - refp[b, :n][sel]
             print(f"[{case}] batch {bi} utt {b}: log-prob max abs diff {np.abs(diff).max():.3f}, "
@@ -367,7 +367,7 @@ def test_transcribe_api_surface(asr, golden_cases, model_dirs, case):
 
 @pytest.mark.parametrize("case", ["causal_ln", "sym_bn"])
 def test_bounded_context_encoder_vs_reference_fixture(asr, golden_cases, case):
-    """decoding_chunk_size > 0: chunk-masked attention (utils/mask.py:88-197) inside the tcgen05 attention kernel;
+    """decoding_chunk_size > 0: chunk-masked attention (utils/mask.py:88-197) inside the wgmma attention kernel;
     encoder_out vs the live-reference fixture with the same bf16 tolerance as the full-context encoder, and the
     chunked output must differ from the full-context one (the mask is really applied)."""
     import json as _json

@@ -1,4 +1,4 @@
-"""Encoder-shaped attention micro-benchmark: tcgen05 kernel (incl. the K''/bias pre-kernel) vs the mma.sync kernel."""
+"""Encoder-shaped attention micro-benchmark: wgmma kernel (incl. the K''/bias pre-kernel) vs the mma.sync kernel."""
 import ctypes as C, json, math, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

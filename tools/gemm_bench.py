@@ -1,4 +1,4 @@
-"""Per-shape timing of the tcgen05 GEMM kernel through the C ABI (CUDA events, warm, L2-cold-ish: operands >> L2)."""
+"""Per-shape timing of the wgmma GEMM kernel through the C ABI (CUDA events, warm, L2-cold-ish: operands >> L2)."""
 import ctypes as C
 import json
 import sys

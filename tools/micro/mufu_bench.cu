@@ -1,5 +1,5 @@
 // Micro-benchmark: MUFU.EX2 throughput per SM (and with interleaved FFMA), to size the softmax loop of attention_tc.cu.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/mufu_bench tools/micro/mufu_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/mufu_bench tools/micro/mufu_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,4 +1,4 @@
-"""Drop-in import name: `import wenet; wenet.load_model(...)` resolves to the B200 engine.
+"""Drop-in import name: `import wenet; wenet.load_model(...)` resolves to the H100 engine.
 
 The reference installs its package as `wenet` (pyproject.toml:25-32); code written against it
 (`wenet.load_model`, `wenet.ReverbASR`, `wenet.get_available_models`, `wenet.download_model`,
