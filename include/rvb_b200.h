@@ -207,6 +207,42 @@ RVB_API int rvb_decoder_step_logp(rvb_model* m, const float* d_enc_out, const in
                                   const int* h_hyps, int L, const float* h_cat_embs, int n_cat, float* h_logp,
                                   void* stream);
 
+/* ---- CTC forced alignment of a known transcript (force_align, utils/ctc_utils.py:95-161; driver bin/alignment.py) ----
+ * Viterbi over the states [b, y0, b, y1, ..., y_{U-1}, b] in fp32 with the reference's tie rules (stay, then s-1, then
+ * s-2; end state S-1 unless S-2 is strictly better): the frame alignment is the reference's, bit for bit.
+ * Batched form, B utterances that each fit one chunk: d_logp (B*Tp, V) fp32 log-probs (rvb_ctc_topk's d_logp),
+ * h_labels (B, max_U) / h_label_lens (B).  Host outputs: h_frames (B, Tp) the token id of every frame (blank_id or a
+ * label; -1 from h_enc_lens[b] on), h_first / h_last / h_peak (B, max_U) first, last and peak frame of every label (peak =
+ * the frame of its span with the largest log-prob, first on ties), h_peak_logp (B, max_U) that log-prob, h_score (B)
+ * the Viterbi score, h_loglik (B) log p(y | x) by the forward algorithm in float64 (NULL: skipped).
+ * An alignment exists iff U >= 1 and enc_len >= U + #(adjacent equal labels); an empty or infeasible label sequence, a
+ * label that is blank or >= V, or U > 12287 fails on the host, before any launch, naming the utterance. */
+RVB_API int rvb_ctc_force_align(const float* d_logp, int V, const int* h_enc_lens, int B, int Tp, const int* h_labels,
+                                const int* h_label_lens, int max_U, int blank_id, int* h_frames, int* h_first,
+                                int* h_last, int* h_peak, float* h_peak_logp, float* h_score, double* h_loglik,
+                                void* stream);
+
+/* Resumable form, ONE trellis fed piecewise — what carries a transcript across the independent encoder chunks of a long
+ * recording; any split of the rows gives exactly the result of a single push.
+ *   begin   labels, the total number of frames that will be pushed, and a budget: the handle owns
+ *           rvb_aligner_workspace_bytes() of device memory — per frame and label slot (U + 1 rounded up to 128, or to
+ *           768 above 4095 labels) 1 byte of back-pointers and 4 bytes of emission log-prob, i.e. about
+ *           5 * total_frames * (U + 1) bytes: 5.6 GB for one hour (90 500 frames) against 12 000 tokens.  A request
+ *           over budget_bytes (> 0) fails before anything is allocated.  m may be NULL; with a model the trellis runs on
+ *           the model's search side stream, so that it hides under the next encoder pass on `stream`.
+ *   push    n_rows further rows of (n_rows, V) log-probs: only the valid frames of a chunk.  The rows are consumed in
+ *           stream order on `stream` (they may be overwritten by later work on it); nothing is synchronised.
+ *   finish  frames indexed over the whole recording, outputs as above with B = 1, Tp = total_frames, max_U = U;
+ *           synchronises, then frees the handle — also when it fails.  abort frees a handle that will not be finished. */
+typedef struct rvb_aligner rvb_aligner;
+RVB_API long long rvb_aligner_workspace_bytes(int U, int total_frames, int want_loglik);
+RVB_API rvb_aligner* rvb_aligner_begin(rvb_model* m, const int* h_labels, int U, int total_frames, int V, int blank_id,
+                                       int want_loglik, long long budget_bytes, void* stream);
+RVB_API int rvb_aligner_push(rvb_aligner* a, const float* d_logp, int n_rows, void* stream);
+RVB_API int rvb_aligner_finish(rvb_aligner* a, int* h_frames, int* h_first, int* h_last, int* h_peak, float* h_peak_logp,
+                               float* h_score, double* h_loglik, void* stream);
+RVB_API void rvb_aligner_abort(rvb_aligner* a);
+
 /* ---- kernel-level entry points (parity tests, profiling) ----------------------------------------------------- */
 /* C[M,N] = A[M,K] W[N,K]^T + bias; act: 0 none 1 relu 2 silu 3 glu; out_mode: 0 bf16, 1 f32, 2 f32 residual += alpha*(.)
  * act 3 (pointwise_conv1 + GLU of the conformer conv module, convolution.py:129-130): bf16 output (M, N/2); W / bias

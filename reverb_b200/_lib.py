@@ -76,6 +76,12 @@ SIGNATURES = {
     "rvb_decoder_cache_end": (_i, [_vp]),
     "rvb_decoder_step_logp": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp, _vp]),
     "rvb_attention_rescoring": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp]),
+    "rvb_ctc_force_align": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rvb_aligner_workspace_bytes": (_ll, [_i, _i, _i]),
+    "rvb_aligner_begin": (_vp, [_vp, _vp, _i, _i, _i, _i, _i, _ll, _vp]),
+    "rvb_aligner_push": (_i, [_vp, _vp, _i, _vp]),
+    "rvb_aligner_finish": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rvb_aligner_abort": (None, [_vp]),
     "rvb_gemm_bf16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _i, _vp]),
     "rvb_gemm_bf16x3": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _i, _vp]),
     "rvb_f32_to_bf16_pair": (_i, [_vp, _vp, _ll, _i, _vp]),

@@ -9,6 +9,7 @@ plan (reverb_b200/engine.py) instead of a torch.nn graph:
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -22,6 +23,17 @@ from .search import (DecodeResult, attention_beam_search, ctc_prefix_beam_search
 SUPPORTED_METHODS = ("attention", "ctc_greedy_search", "ctc_prefix_beam_search", "attention_rescoring", "joint_decoding")
 JOINT_DECODING_SOS = 10000        # hard-coded in the reference (transformer/search.py:480)
 JOINT_PRE_BEAM_RATIO = 1.5        # joint_decoding's default (search.py:457)
+
+
+def alignment_result(a) -> DecodeResult:
+    """engine.Alignment -> DecodeResult with `times` / `tokens_confidence` filled, so that it renders like a search
+    result; the frame-level alignment travels as extra attributes."""
+    T = len(a.frames)
+    r = DecodeResult(tokens=list(a.tokens), score=float(a.score), confidence=math.exp(float(a.score) / T),
+                     tokens_confidence=[math.exp(float(x)) for x in a.peak_logp], times=[int(t) for t in a.peak])
+    r.alignment = a.frames
+    r.first_frames, r.last_frames, r.loglik = a.first, a.last, a.loglik
+    return r
 
 
 class ASRModel:
@@ -250,6 +262,26 @@ class ASRModel:
         finally:
             for st in inflight:          # only non-empty when a stage raised or the consumer stopped early
                 self.engine.ticket_release(st["ticket"])
+
+    @torch.no_grad()
+    def align(self, speech: torch.Tensor, speech_lengths, tokens, token_lengths, blank_id: int = 0, cat_embs=None,
+              blank_penalty: float = 0.0, want_loglik: bool = False) -> List[DecodeResult]:
+        """CTC forced alignment of known transcripts (the reference's force_align, utils/ctc_utils.py:105-161, driven by
+        bin/alignment.py one utterance at a time): encoder -> CTC log-probs -> batched Viterbi on the GPU (csrc/align.cu).
+        tokens (B, max_U) padded ids, token_lengths (B).  One DecodeResult per utterance: `tokens`, `times` = the peak
+        frame of every token (the frame of its span with the largest log-prob: the prefix search's notion of a token
+        time), `tokens_confidence` = exp(peak log-prob), `score` = Viterbi score, `confidence` = exp(score / T); plus
+        `alignment` (the token id of every frame), `first_frames` / `last_frames` and, when asked for, `loglik`.
+        ValueError when a transcript is empty or has more tokens (+ repeats) than the audio has encoder frames."""
+        if not speech.is_cuda:
+            speech = speech.to(self.engine.device, non_blocking=True)
+        tok = np.asarray(tokens.cpu() if torch.is_tensor(tokens) else tokens)
+        ulen = np.asarray(token_lengths.cpu() if torch.is_tensor(token_lengths) else token_lengths).reshape(-1)
+        labels = [[int(x) for x in tok[b][:int(ulen[b])]] for b in range(speech.shape[0])]
+        encoder_out, encoder_lens = self._forward_encoder(speech.to(torch.float32), speech_lengths, cat_embs)
+        logp = self.ctc_logprobs(encoder_out, blank_penalty, blank_id)
+        return [alignment_result(a) for a in
+                self.engine.force_align(logp, encoder_lens, labels, blank_id, want_loglik)]
 
     def attention_rescoring(self, prefix_results: List[DecodeResult], encoder_out: torch.Tensor, encoder_lens,
                             ctc_weight: float = 0.0, reverse_weight: float = 0.0, cat_embs=None) -> List[DecodeResult]:

@@ -1581,6 +1581,12 @@ struct SearchTicket {
   }
 };
 
+int search_side_stream(rvb_model* m, cudaStream_t* out) {
+  if (m->s_search == nullptr) RVB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->s_search, cudaStreamNonBlocking));
+  *out = m->s_search;
+  return 0;
+}
+
 static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val, const int* d_topk_idx, int k,
                          const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int beam, int blank_id,
                          DevBuf& ws, cudaStream_t stream) {

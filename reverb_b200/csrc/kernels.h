@@ -3,7 +3,13 @@
 #pragma once
 #include "common.cuh"
 
+struct rvb_model;
+
 namespace rvb {
+
+// the side stream the prefix beam search runs on (engine.cu search_submit), created on first use; forced alignment
+// (align.cu) puts its serial trellis there too
+int search_side_stream(::rvb_model* m, cudaStream_t* out);
 
 // ------------------------------------------------------------------ GEMM (gemm.cu)
 // ACT_GLU (bf16 output only): the N = 2C weight rows are interleaved in groups of 32 — rows [64j, 64j+32) are the

@@ -71,6 +71,69 @@ def ctc_align(tokens, times, confidences: Optional[List[float]], tokenizer, fram
     return words
 
 
+def frames_to_ms(frames, chunk_frames, chunk_ms: int, frame_shift_ms: int) -> List[int]:
+    """Frames counted over the VALID encoder frames of consecutive chunks -> milliseconds in the recording.
+    chunk_frames[c] = valid frames of chunk c.  Frame j of chunk c sits at c * chunk_ms + j * frame_shift_ms: chunks
+    are cut in input frames, and a chunk's encoder frames do not fill it (748 x 40 ms in a 29.98 s chunk), so one
+    global multiplication by frame_shift_ms would drift."""
+    starts, total = [], 0
+    for n in chunk_frames:
+        starts.append(total)
+        total += int(n)
+    out, c = [], 0
+    for f in frames:
+        f = int(f)
+        assert 0 <= f < total
+        if f < starts[c]:
+            c = 0
+        while c + 1 < len(starts) and f >= starts[c + 1]:
+            c += 1
+        out.append(c * chunk_ms + (f - starts[c]) * frame_shift_ms)
+    return out
+
+
+def ctc_align_ms(tokens, times_ms, confidences: Optional[List[float]], tokenizer, frame_shift_ms: int) -> List[Dict[str, Any]]:
+    """ctc_align() for ONE token sequence whose peaks are given in milliseconds of the whole recording (forced alignment
+    of a transcript across chunks): a word whose pieces fall on both sides of a chunk boundary stays one word.  Same
+    word rules; with all peaks in one chunk it returns what ctc_align(..., time_shift_ms = the chunk's start) does, except
+    that a word's 100 ms lead-in is clamped at the start of the recording only, not at the start of every chunk."""
+    if len(tokens) != len(times_ms):
+        raise AssertionError("ctc_align_ms needs one timestamp per token")
+    n = len(tokens)
+    pieces = [tokenizer.detokenize([t])[1][0] for t in tokens]
+    words: List[Dict[str, Any]] = []
+    text, ids, start, first = "", [], -1, -1
+
+    def midpoint(a: int, b: int) -> int:      # (t_a + t_b) // 2 * frame_shift_ms, written on milliseconds
+        return a + (b - a) // (2 * frame_shift_ms) * frame_shift_ms
+
+    def end_time(i: int) -> int:
+        if i < n - 1 and times_ms[i + 1] - times_ms[i] < GAP_MS:
+            return midpoint(times_ms[i], times_ms[i + 1])
+        return times_ms[i]
+
+    def conf(lo: int, hi: int):
+        return max(confidences[lo:hi + 1]) if confidences else 0
+
+    for i in range(n):
+        piece = pieces[i]
+        nxt = pieces[i + 1] if i + 1 < n else SPACE
+        text += piece[len(SPACE):] if piece.find(SPACE) != -1 else piece
+        ids.append(tokens[i])
+        if start == -1:
+            start = max(times_ms[i] - GAP_MS, 0)
+            if i > 0 and times_ms[i] - times_ms[i - 1] < GAP_MS:
+                start = midpoint(times_ms[i - 1], times_ms[i])
+            first = i
+        special = text not in ("", SPACE) and _is_special(text)
+        if special or _starts_word(nxt) or _is_special(nxt):
+            if text not in ("", SPACE):
+                words.append({"word": text, "unit_id": ids[0] if special else -1, "start_time_ms": start,
+                              "end_time_ms": end_time(i), "confidence": conf(first, i), "unit_ids": ids})
+            text, ids, start, first = "", [], -1, 0
+    return words
+
+
 def adjust_model_time_offset(words: List[Dict[str, Any]], adjustment):
     """Move every word earlier by min(adjustment, gap to the previous word's end).  Like the reference
     (ctc_align.py:117-118) an adjustment of 0 returns None."""

@@ -475,5 +475,124 @@ class Engine:
         return self.rescoring_scores_raw(enc_out, enc_lens, toks, hlen, cat_embs, reverse_weight)
 
 
+    # ---- CTC forced alignment (csrc/align.cu; include/rvb_b200.h rvb_ctc_force_align / rvb_aligner_*)
+    def force_align(self, logp: torch.Tensor, enc_lens, labels: Sequence[Sequence[int]], blank_id: int = 0,
+                    want_loglik: bool = False) -> List["Alignment"]:
+        """logp (B, Tp, V) fp32 log-probs on the device, one label list per utterance -> one Alignment each."""
+        assert logp.is_cuda and logp.dtype == torch.float32 and logp.dim() == 3
+        logp = logp.contiguous()
+        B, Tp, V = logp.shape
+        lens = np.ascontiguousarray(np.asarray(enc_lens, dtype=np.int32).reshape(-1))
+        assert lens.shape[0] == B and len(labels) == B
+        for b in range(B):
+            check_alignable(labels[b], int(lens[b]), f"utterance {b}")
+        ulen = np.asarray([len(y) for y in labels], dtype=np.int32)
+        max_U = int(ulen.max())
+        lab = np.zeros((B, max_U), dtype=np.int32)
+        for b, y in enumerate(labels):
+            lab[b, :len(y)] = np.asarray(y, dtype=np.int32)
+        out = _AlignBuffers(B, Tp, max_U, want_loglik)
+        with torch.cuda.device(self.device):
+            check(self.lib.rvb_ctc_force_align(_ptr(logp), V, _np_ptr(lens), B, Tp, _np_ptr(lab), _np_ptr(ulen), max_U,
+                                               int(blank_id), *out.pointers(), self._stream()), "rvb_ctc_force_align")
+        return [out.alignment(b, labels[b], int(lens[b])) for b in range(B)]
+
+    def aligner(self, labels: Sequence[int], total_frames: int, blank_id: int = 0, want_loglik: bool = False,
+                budget_bytes: int = 0, side_stream: bool = True) -> "Aligner":
+        """One trellis over `total_frames` frames, fed piecewise (Aligner.push) — the form that crosses the encoder
+        batches of a long recording.  budget_bytes > 0 bounds the device workspace (Aligner.workspace_bytes)."""
+        return Aligner(self, labels, total_frames, blank_id, want_loglik, budget_bytes, side_stream)
+
+
+class Alignment:
+    """Forced alignment of one label sequence: `frames` the token id of every frame (what the reference's force_align
+    returns), per label its `first` / `last` / `peak` frame and `peak_logp`, the Viterbi `score` (float32) and, when
+    asked for, `loglik` = log p(y | x)."""
+
+    def __init__(self, tokens, frames, first, last, peak, peak_logp, score, loglik=None):
+        self.tokens, self.frames, self.first, self.last, self.peak = tokens, frames, first, last, peak
+        self.peak_logp, self.score, self.loglik = peak_logp, score, loglik
+
+
+def check_alignable(labels: Sequence[int], n_frames: int, what: str = "transcript") -> None:
+    """An alignment exists iff U >= 1 and T >= U + #(adjacent equal labels): a repeat needs a blank frame in between."""
+    U = len(labels)
+    if U == 0:
+        raise ValueError(f"reverb_b200: {what} is empty, nothing to align")
+    need = U + sum(1 for a, b in zip(labels[:-1], labels[1:]) if a == b)
+    if n_frames < need:
+        raise ValueError(f"reverb_b200: {what} is infeasible: {U} tokens need at least {need} encoder frames, "
+                         f"the audio has {n_frames}")
+
+
+class _AlignBuffers:
+    def __init__(self, B: int, T: int, max_U: int, want_loglik: bool):
+        self.frames = np.zeros((B, T), dtype=np.int32)
+        self.first, self.last, self.peak = (np.zeros((B, max_U), dtype=np.int32) for _ in range(3))
+        self.peak_logp = np.zeros((B, max_U), dtype=np.float32)
+        self.score = np.zeros(B, dtype=np.float32)
+        self.loglik = np.zeros(B, dtype=np.float64) if want_loglik else None
+
+    def pointers(self):
+        return [_np_ptr(a) for a in (self.frames, self.first, self.last, self.peak, self.peak_logp, self.score,
+                                     self.loglik)]
+
+    def alignment(self, b: int, labels, T: int) -> Alignment:
+        U = len(labels)
+        return Alignment(list(labels), self.frames[b, :T].copy(), self.first[b, :U].copy(), self.last[b, :U].copy(),
+                         self.peak[b, :U].copy(), self.peak_logp[b, :U].copy(), np.float32(self.score[b]),
+                         None if self.loglik is None else float(self.loglik[b]))
+
+
+class Aligner:
+    """Handle of the resumable alignment (rvb_aligner_*).  push() enqueues and returns; finish() synchronises."""
+
+    def __init__(self, engine: Engine, labels: Sequence[int], total_frames: int, blank_id: int, want_loglik: bool,
+                 budget_bytes: int, side_stream: bool):
+        self.engine, self.labels, self.total = engine, [int(t) for t in labels], int(total_frames)
+        self.want_loglik = bool(want_loglik)
+        check_alignable(self.labels, self.total)
+        lab = np.ascontiguousarray(self.labels, dtype=np.int32)
+        self._h = None
+        with torch.cuda.device(engine.device):
+            h = engine.lib.rvb_aligner_begin(engine._h if side_stream else None, _np_ptr(lab), len(self.labels),
+                                             self.total, engine.vocab, int(blank_id), int(self.want_loglik),
+                                             int(budget_bytes), engine._stream())
+        if not h:
+            raise RuntimeError("rvb_aligner_begin failed: " + _lib.last_error())
+        self._h = C.c_void_p(h)
+
+    @staticmethod
+    def workspace_bytes(n_labels: int, total_frames: int, want_loglik: bool = False) -> int:
+        return int(_lib.load().rvb_aligner_workspace_bytes(int(n_labels), int(total_frames), int(want_loglik)))
+
+    def push(self, logp_rows: torch.Tensor) -> None:
+        """(n, V) fp32 log-probs of the next n frames, on the device."""
+        assert logp_rows.is_cuda and logp_rows.dtype == torch.float32 and logp_rows.dim() == 2
+        assert logp_rows.shape[1] == self.engine.vocab
+        rows = logp_rows.contiguous()
+        with torch.cuda.device(self.engine.device):
+            check(self.engine.lib.rvb_aligner_push(self._h, _ptr(rows), rows.shape[0], self.engine._stream()),
+                  "rvb_aligner_push")
+
+    def finish(self) -> Alignment:
+        out = _AlignBuffers(1, self.total, len(self.labels), self.want_loglik)
+        h, self._h = self._h, None                     # the native call frees the handle, also when it fails
+        with torch.cuda.device(self.engine.device):
+            check(self.engine.lib.rvb_aligner_finish(h, *out.pointers(), self.engine._stream()), "rvb_aligner_finish")
+        return out.alignment(0, self.labels, self.total)
+
+    def abort(self) -> None:
+        if self._h is not None:
+            self.engine.lib.rvb_aligner_abort(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.abort()
+        except Exception:
+            pass
+
+
 def launch_count() -> int:
     return int(_lib.load().rvb_launch_count())

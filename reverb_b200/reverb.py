@@ -26,9 +26,9 @@ import torch
 import torch.nn.functional as F
 import yaml
 
-from .asr_model import ASRModel
-from .ctc_align import adjust_model_time_offset, ctc_align, hyps_to_ctm, hyps_to_txt
-from .engine import Engine, check_beam_size
+from .asr_model import ASRModel, alignment_result
+from .ctc_align import adjust_model_time_offset, ctc_align, ctc_align_ms, frames_to_ms, hyps_to_ctm, hyps_to_txt
+from .engine import Engine, check_alignable, check_beam_size
 from .search import DecodeResult
 from .text import get_blank_id, init_tokenizer
 
@@ -201,6 +201,67 @@ class ReverbASR:
             num_decoding_left_chunks=num_decoding_left_chunks, ctc_weight=ctc_weight,
             simulate_streaming=simulate_streaming, reverse_weight=reverse_weight, blank_penalty=blank_penalty,
             length_penalty=length_penalty, timings_adjustment=timings_adjustment)[0]
+
+
+    def transcript_ids(self, transcript) -> List[int]:
+        """A transcript as token ids: a string goes through the model's sentencepiece pieces (pieces outside the symbol
+        table map to <unk> and are kept, so that every word keeps its place), a list of ids is taken as it is."""
+        if isinstance(transcript, str):
+            ids = self.tokenizer.tokens2ids(self.tokenizer.text2tokens(transcript))
+        else:
+            ids = [int(t) for t in transcript]
+        if len(ids) == 0:
+            raise ValueError("reverb_b200: the transcript is empty, nothing to align")
+        bad = [t for t in ids if t is None or not 0 <= t < len(self.tokenizer.symbol_table) or t == self.blank_id]
+        if bad:
+            raise ValueError(f"reverb_b200: transcript token ids {bad[:5]} are not non-blank ids of the symbol table")
+        return ids
+
+    def align(self, audio_file, transcript, format: str = "ctm", verbatimicity: float = 1.0, chunk_size: int = 2051,
+              batch_size: int = 1, blank_penalty: float = 0.0, timings_adjustment: float = 230) -> str:
+        """Forced alignment of a known transcript (text or token ids) to a recording of any length -> CTM / text.
+        The encoder runs in the usual independent chunks, `batch_size` at a time; the valid log-prob rows of every chunk
+        are pushed into ONE Viterbi trellis (Engine.aligner, on the search side stream, under the next batch's encoder),
+        so the transcript is aligned to the whole recording, with no anchoring."""
+        if format not in ("ctm", "txt"):
+            raise ValueError("Invalid output format.")
+        result, times_ms = self.align_tokens(audio_file, self.transcript_ids(transcript), verbatimicity, chunk_size,
+                                             batch_size, blank_penalty)
+        words = ctc_align_ms(result.tokens, times_ms, result.tokens_confidence, self.tokenizer, self.output_frame_length)
+        if timings_adjustment != 0:
+            words = adjust_model_time_offset(words, timings_adjustment)
+        if format == "txt":
+            return " ".join(hyps_to_txt(words))
+        return "\n".join(hyps_to_ctm(Path(audio_file).name, words))
+
+    def align_tokens(self, audio_file, ids: List[int], verbatimicity: float = 1.0, chunk_size: int = 2051,
+                     batch_size: int = 1, blank_penalty: float = 0.0, want_loglik: bool = False,
+                     workspace_budget_bytes: int = 0) -> Tuple[DecodeResult, List[int]]:
+        """-> (DecodeResult with frames counted over the valid encoder frames of all chunks, per-token peak time in ms)."""
+        fc = self.test_conf["fbank_conf"]
+        feats = self.compute_feats(audio_file, num_mel_bins=fc["num_mel_bins"], frame_length=fc["frame_length"],
+                                   frame_shift=fc["frame_shift"])
+        n = feats.shape[1]
+        feat_lens = [chunk_size] * (n // chunk_size) + ([n % chunk_size] if n % chunk_size else [])
+        chunk_frames = [int(self.engine.lib.rvb_encoder_out_len(fl, chunk_size)) for fl in feat_lens]
+        check_alignable(ids, sum(chunk_frames))
+        cat_embs = torch.tensor([verbatimicity, 1.0 - verbatimicity])
+        aligner = self.engine.aligner(ids, sum(chunk_frames), self.blank_id, want_loglik, workspace_budget_bytes)
+        try:
+            with torch.no_grad():
+                c = 0
+                for feats_batch, feats_lengths in self.feats_batcher(feats, chunk_size, batch_size):
+                    enc_out, enc_lens = self.model._forward_encoder(feats_batch, feats_lengths, cat_embs)
+                    logp = self.model.ctc_logprobs(enc_out, blank_penalty, self.blank_id)
+                    for b in range(logp.shape[0]):
+                        assert int(enc_lens[b]) == chunk_frames[c]
+                        aligner.push(logp[b, :chunk_frames[c]])
+                        c += 1
+            result = alignment_result(aligner.finish())
+        finally:
+            aligner.abort()
+        return result, frames_to_ms(result.times, chunk_frames, chunk_size * self.input_frame_length,
+                                    self.output_frame_length)
 
 
 def get_output(format: str, tokenizer, audio_name: str, hyps: List[DecodeResult], timings_adjustment_ms: int,
