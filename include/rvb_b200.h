@@ -250,6 +250,12 @@ RVB_API void rvb_aligner_abort(rvb_aligner* a);
  * [64j+32, 64j+64) their gates; out[m, c] = value * sigmoid(gate). */
 RVB_API int rvb_gemm_bf16(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act, int out_mode,
                   float alpha, void* d_out, int ldo, void* stream);
+/* For tests and tools: rvb_gemm_bf16 with the row mask the encoder applies internally (not needed to run a model).
+ * Row m is batch m / rows_per_batch, position m % rows_per_batch, and is written only if position < d_row_lens[batch]
+ * (int32, device); masked rows of d_out are left untouched. */
+RVB_API int rvb_gemm_bf16_rows(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act,
+                               int out_mode, float alpha, void* d_out, int ldo, const int* d_row_lens, int rows_per_batch,
+                               void* stream);
 /* The same GEMM in the fp32-accurate "bf16x3" mode (rvb_model_config.precision = 1): d_A (M, 2K) and d_W (N, 2K) hold
  * (hi | lo) bf16 pairs — hi = bf16(v), lo = bf16(v - hi), rvb_f32_to_bf16_pair builds them — and three wgmma passes
  * hi.hi + lo.hi + hi.lo accumulate in fp32.  bf16 outputs (out_mode 0) are written as such a pair too: (M, 2N), or

@@ -2165,6 +2165,26 @@ RVB_API int rvb_gemm_bf16(const void* d_A, const void* d_W, const float* d_bias,
   return rvb::launch_gemm(g, (cudaStream_t)stream);
 }
 
+RVB_API int rvb_gemm_bf16_rows(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act,
+                               int out_mode, float alpha, void* d_out, int ldo, const int* d_row_lens, int rows_per_batch,
+                               void* stream) {
+  rvb::GemmArgs g;
+  g.A = reinterpret_cast<const rvb::bf16*>(d_A);
+  g.W = reinterpret_cast<const rvb::bf16*>(d_W);
+  g.M = M;
+  g.N = N;
+  g.K = K;
+  g.bias = d_bias;
+  g.act = act;
+  g.out_mode = out_mode;
+  g.alpha = alpha;
+  g.out = d_out;
+  g.ldo = ldo;
+  g.row_lens = d_row_lens;
+  g.rows_per_batch = rows_per_batch;
+  return rvb::launch_gemm(g, (cudaStream_t)stream);
+}
+
 RVB_API int rvb_gemm_bf16x3(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act, int out_mode,
                             float alpha, void* d_out, int ldo, void* stream) {
   rvb::GemmArgs g;

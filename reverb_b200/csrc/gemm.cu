@@ -8,12 +8,14 @@
 // Conv2d(d,d,3,stride 2) of Conv2dSubsampling4 (subsampling.py:186-189) as an implicit GEMM whose A tiles are fetched
 // straight out of the channels-last conv1 activation by 4-D TMA boxes (no im2col buffer).
 //
-// Structure per CTA (288 threads, 1 CTA / SM, grid = #SMs, static round-robin tile scheduler), see gemm_wg_kernel:
-//   warp 8 / lane 0 : TMA producer — fills a 4-deep ring of {A 128x64, W BNx64} bf16 tiles (SWIZZLE_128B)
-//   warps 0..7      : two consumer warpgroups, 64 rows each: wgmma m64nBNk16 from shared memory into registers, then
-//                     the fused epilogue (bias / ReLU / SiLU / GLU / residual(+row mask) / log-sum-exp / rel-pos keys)
-//                     on a shared-memory copy of the accumulator; outputs pass through a warp-private XOR-swizzled
-//                     staging tile so global accesses are coalesced.
+// Structure per CTA (384 threads, 1 CTA / SM, grid = #SMs, static round-robin tile scheduler), see gemm_wg_kernel:
+//   warpgroup 0    : TMA producer (one thread, 40 registers) — fills a 4-deep ring of {A 128x64, W BNx64} bf16 tiles
+//                    (SWIZZLE_128B)
+//   warpgroups 1-2 : ping-pong consumers (232 registers), alternate whole tiles: wgmma m64nBNk16 x 2 from shared memory
+//                    into registers, then — while the other warpgroup runs the next tile's MMAs — the fused epilogue
+//                    (bias / ReLU / SiLU / GLU / residual(+row mask) / log-sum-exp / rel-pos keys) on a shared-memory
+//                    copy of the accumulator; outputs pass through a per-warp XOR-swizzled staging tile so global
+//                    accesses are coalesced.
 // Tuning aid (environment, read once): RVB_GEMM_SKIP_EPI=1|2|3 (main loop only / no global stores / accumulator
 // reads + math only — results are wrong by construction; tools/gemm_bench.py).  RVB_GEMM=simt selects the CUDA-core
 // bring-up kernel, RVB_GEMM=narrow 64-wide tiles wherever the epilogue allows them.
@@ -675,28 +677,41 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
   }
 }
 
-// warps 0..7: two consumer warpgroups (wgmma on 64 rows each, then the epilogue of those rows), warp 8: TMA producer
+// warpgroup 0: TMA producer (one thread), warpgroups 1-2: consumers, each owning whole 128 x BN tiles in turn
 constexpr int kConsumerWGs = 2;
-constexpr int kGemmThreads = 128 * kConsumerWGs + 32;
+constexpr int kGemmThreads = 128 * (1 + kConsumerWGs);
+// setmaxnreg budgets: 40 * 128 + 232 * 256 = 64 512 of the SM's 65 536 registers
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
+  // 4 stages + the whole 64 KB accumulator tile.  A 5th stage fits only with the tile copied and drained one 64-row half
+  // at a time; measured on the H100 that is slower (DESIGN.md §4): the drain loses half its parallelism and the second
+  // half's accumulators stay live (and spill) through the first half's drain.
   static constexpr int STAGES = 4;
   static constexpr uint32_t A_BYTES = BM * BK * 2;
   static constexpr uint32_t B_BYTES = BN * BK * 2;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t ACC_BYTES = BM * BN * 4;   // fp32 accumulator tile (epilogue copy)
-  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 8 * 4096 /*epilogue staging*/ + 256 /*barriers*/ +
-                                         1024 /*align slack*/;
+  static constexpr uint32_t ACC_BYTES = BM * BN * 4;   // fp32 accumulator tile (epilogue copy), shared by both consumers
+  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 4 * 4096 /*epilogue staging, 4 warps*/ +
+                                         256 /*barriers*/ + 1024 /*align slack*/;
 };
 
 // Persistent, warp-specialised TMA + wgmma GEMM (1 CTA / SM, grid = min(#tiles, #SMs), static round-robin tiles of
-// 128 x BN).  The producer fills a STAGES-deep ring of {A 128x64, W BNx64} bf16 tiles (SWIZZLE_128B).  Consumer
-// warpgroup g multiplies rows [64g, 64g+64) of every stage with 4 x wgmma m64nBNk16, releasing the previous stage as
-// soon as its MMAs have retired, then copies its accumulator to shared memory and drains it through the fused epilogue
-// (drain_tile) while the producer already streams the next tile's first stages.
+// 128 x BN), with ping-pong consumer warpgroups.  The producer fills a STAGES-deep ring of {A 128x64, W BNx64} bf16
+// tiles (SWIZZLE_128B) in the CTA's tile order.  The CTA's i-th tile belongs to consumer warpgroup i % 2, which
+// multiplies the whole tile (2 x wgmma m64nBNk16 per k16 step, rows 0-63 and 64-127), releasing each stage as soon as
+// its MMAs have retired, then copies its accumulator to the shared fp32 tile and drains it through the fused epilogue
+// (drain_tile) while the other warpgroup already runs the next tile's MMAs.  Two pairs of mbarriers order the hand-offs:
+//   turn[w]    : warpgroup w may start its K loop — the other one has issued the last MMA of the previous tile;
+//   accfree[w] : warpgroup w may write the shared accumulator tile — the other one has drained the previous tile.
+// Both are arrived by all 128 threads of the other warpgroup once per tile, so the CTA's tile i (i >= 1) waits for
+// completion (i + 1) / 2 of its barrier, parity ((i - 1) / 2) & 1; tile 0 waits for nothing.  Because a warpgroup
+// arrives only after it has itself waited for the previous completion, a barrier is never more than one phase ahead
+// of its waiter.  Arrivals no tile waits for (the CTA's last tile, a warpgroup without tiles) are harmless.
 template <int BN, int EPI, bool PAIR>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
@@ -708,9 +723,11 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
   float* accs = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
   float* stage_epi = accs + Cfg::BM * BN;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_epi + 8 * 1024);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_epi + 4 * 1024);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
+  uint64_t* turn = bars + 2 * STAGES;
+  uint64_t* accfree = turn + 2;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -718,7 +735,11 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 4 * kConsumerWGs);   // lane 0 of every consumer warp
+      mbar_init(&empty[i], 4);   // lane 0 of every warp of the consuming warpgroup
+    }
+    for (int w = 0; w < kConsumerWGs; ++w) {
+      mbar_init(&turn[w], 128);
+      mbar_init(&accfree[w], 128);
     }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
@@ -727,9 +748,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
   const int nkb = p.num_k_blocks;
 
-  if (warp == 4 * kConsumerWGs) {
+  if (warp < 4) {
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
       uint32_t stage = 0, phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         TileCoord t = decode_tile(p, tile, BN);
@@ -759,37 +781,43 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   } else {
     // ------------------------------------------------------------ consumer warpgroups
-    const int wg = warp >> 2, wl = warp & 3;
-    const int q = 2 * wg + (wl & 1);   // 32-row quarter of the tile this warp drains
-    const int chalf = wl >> 1;         // which half of the accumulator columns
-    // LSE partials and the coalesced GLU path work on 128-column slabs and the bf16 path on 64-column chunks: there (and
-    // for 64-wide tiles) one warp per row quarter takes all columns
-    constexpr bool whole = (EPI == EPI_LSE || EPI == EPI_GLU || BN == 64);
-    const int c0 = whole ? (chalf ? BN : 0) : chalf * (BN / 2);
-    const int c1 = whole ? BN : c0 + BN / 2;
-    float* stage_w = stage_epi + warp * 1024;
-    uint32_t stage = 0, phase = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    // one warpgroup drains at a time: warp wl takes rows [32 wl, 32 wl + 32) and all columns
+    float* stage_w = stage_epi + wl * 1024;
+    float acc[BN];   // rows 0-63 in acc[0, BN/2), rows 64-127 in acc[BN/2, BN) (wgmma fragment layout, common.cuh)
+    for (int i = wg; blockIdx.x + i * gridDim.x < p.num_tiles; i += kConsumerWGs) {
+      const int tile = blockIdx.x + i * gridDim.x;
       TileCoord t = decode_tile(p, tile, BN);
+      // the ring is consumed in the CTA's tile order: tile i's k-blocks are ring uses [i * nkb, (i + 1) * nkb)
+      const uint32_t u0 = (uint32_t)i * (uint32_t)nkb;
+      uint32_t stage = u0 % STAGES, phase = (u0 / STAGES) & 1;
+      const uint32_t hand_parity = ((i - 1) >> 1) & 1;   // see the comment above the kernel
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int e = 0; e < BN; ++e) acc[e] = 0.f;
+      if (i > 0) mbar_wait(&turn[wg], hand_parity);
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full[stage], phase);
-        const uint64_t adesc = make_sw128_desc(smem_u32(sA + stage * Cfg::A_BYTES + wg * (Cfg::A_BYTES / 2)));
+        const uint64_t adesc = make_sw128_desc(smem_u32(sA + stage * Cfg::A_BYTES));
         const uint64_t bdesc = make_sw128_desc(smem_u32(sB + stage * Cfg::B_BYTES));
-        wgmma_fence_regs<BN / 2>(acc);
+        constexpr uint64_t kHalfA = (Cfg::A_BYTES / 2) >> 4;   // rows 64-127 of the A stage, in descriptor units
+        wgmma_fence_regs<BN>(acc);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           // advance 16 bf16 = 32 B along K inside the 128 B swizzle span: +2 in the (addr >> 4) field
-          if constexpr (BN == 128) wgmma_m64n128k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
-          else wgmma_m64n64k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+          if constexpr (BN == 128) {
+            wgmma_m64n128k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+            wgmma_m64n128k16_ss(acc + BN / 2, adesc + kHalfA + 2 * k, bdesc + 2 * k, 1u);
+          } else {
+            wgmma_m64n64k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+            wgmma_m64n64k16_ss(acc + BN / 2, adesc + kHalfA + 2 * k, bdesc + 2 * k, 1u);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();   // the previous stage's MMAs have retired: hand its buffers back to the producer
-        wgmma_fence_regs<BN / 2>(acc);
+        wgmma_fence_regs<BN>(acc);
         if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
         prev = (int)stage;
         if (++stage == STAGES) {
@@ -797,26 +825,29 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           phase ^= 1;
         }
       }
+      mbar_arrive(&turn[wg ^ 1]);   // every MMA of this tile is issued: the other warpgroup's K loop may follow
       wgmma_wait<0>();
-      wgmma_fence_regs<BN / 2>(acc);
+      wgmma_fence_regs<BN>(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-      // accumulator -> shared memory (this warpgroup's 64 rows; the previous tile's drain of them is finished)
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-      {
-        const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+      // accumulator -> shared memory, once the other warpgroup has drained the previous tile out of it
+      if (i > 0) mbar_wait(&accfree[wg], hand_parity);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r0 = h * 64 + wl * 16 + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int c = 8 * j + 2 * (lane & 3);
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int r = r0 + 8 * i;
+          for (int e = 0; e < 2; ++e) {
+            const int r = r0 + 8 * e;
             *reinterpret_cast<float2*>(accs + r * BN + ((((c >> 2)) ^ (r & 7)) << 2) + (c & 3)) =
-                make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+                make_float2(acc[h * (BN / 2) + 4 * j + 2 * e], acc[h * (BN / 2) + 4 * j + 2 * e + 1]);
           }
         }
       }
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-      drain_tile<BN, EPI, PAIR>(p, t, q, lane, accs, c0, c1, stage_w);
+      drain_tile<BN, EPI, PAIR>(p, t, wl, lane, accs, 0, BN, stage_w);
+      mbar_arrive(&accfree[wg ^ 1]);   // this thread's reads of the tile and of its staging slot are done
     }
   }
 }

@@ -1,8 +1,9 @@
 """Per-shape timing of the wgmma GEMM kernel through the C ABI (CUDA events, warm, L2-cold-ish: operands >> L2)."""
 import ctypes as C
 import json
-import sys
 import os
+import subprocess
+import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -48,10 +49,18 @@ def bench(M, N, K, act, out_mode, iters=10):
             "cublas_ms": round(ms_cb, 4), "cublas_tflops": round(2.0 * M * N * K / (ms_cb * 1e-3) / 1e12, 1)}
 
 
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                        str(torch.cuda.current_device())], capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name()
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "one":       # single shape, for ncu captures
         print(json.dumps(bench(47872, 4096, 1024, 2, 0, iters=3)))
         sys.exit(0)
+    print(json.dumps({"card": card(), "lib": os.environ.get("RVB_LIB_PATH") or "in-tree",
+                      "skip_epi": os.environ.get("RVB_GEMM_SKIP_EPI", "0")}), flush=True)
     M = 47872
     shapes = [(M, 4096, 1024, 2, 0), (M, 1024, 4096, 0, 2), (M, 3072, 1024, 0, 0), (M, 1024, 1024, 0, 2),
               (M, 2048, 1024, 0, 0), (M, 10001, 1024, 0, 1), (M * 19, 1024, 1024, 1, 0), (M, 1024, 19456, 0, 1),
