@@ -10,6 +10,7 @@
  *   rvb_ctc_topk                <- ASRModel.ctc_logprobs + logp.topk        asr_model.py:318-329, search.py:111,155
  *   rvb_ctc_greedy_search       <- ctc_greedy_search                        transformer/search.py:106-121
  *   rvb_ctc_prefix_beam_search  <- ctc_prefix_beam_search                   transformer/search.py:124-248
+ *   rvb_context_graph_*, *_biased <- ContextGraph + its search branches      utils/context_graph.py, search.py:124-248
  *   rvb_attention_rescoring     <- forward_attention_decoder + the gather   asr_model.py:868-978, search.py:410-436
  *   rvb_beam_search_rescoring   <- the two calls above back to back          asr_model.py:403-424 (n-best stays on the device)
  *   rvb_decoder_step_topk       <- decoder.forward_one_step + logp.topk     search.py:302-306 (`attention` mode)
@@ -136,6 +137,27 @@ RVB_API int rvb_ctc_prefix_beam_search(const float* d_topk_val, const int* d_top
                                int Tp, int beam, int blank_id, int max_len, int* h_tokens, int* h_times, int* h_lens,
                                double* h_scores, int* h_nhyp, void* stream);
 
+/* ---- context biasing (utils/context_graph.py ContextGraph + the `context_graph` branches of search.py:124-248) ----
+ * A graph is uploaded once and used read-only by any number of searches.  Tables (reverb_b200.context_graph
+ * device_tables builds them from either graph form): n_nodes states, 0 = root; the children of state s are the edges
+ * [h_child_off[s], h_child_off[s+1]) with tokens h_child_tok (strictly increasing within a state) and target states
+ * h_child_dst (n_nodes - 1 edges: a trie); h_fail (n_nodes) fail links; h_bonus = node_score, h_emit = output_score,
+ * h_token_score = token_score, float64.  Checked before anything is allocated: a trie reachable from the root, tokens in
+ * [0, vocab) and != blank_id, fail links to strictly shallower states, finite scores; NULL + rvb_last_error() otherwise.
+ * destroy waits for the searches enqueued with the graph, then frees it. */
+typedef struct rvb_context_graph rvb_context_graph;
+RVB_API rvb_context_graph* rvb_context_graph_create(int n_nodes, const int* h_child_off, const int* h_child_tok,
+                                                    const int* h_child_dst, const int* h_fail, const double* h_bonus,
+                                                    const double* h_emit, const double* h_token_score, int vocab,
+                                                    int blank_id);
+RVB_API void rvb_context_graph_destroy(rvb_context_graph* g);
+/* rvb_ctc_prefix_beam_search with context biasing: prefixes are ranked by score + context score; h_scores receives
+ * score - node_score of the prefix's final state (the reference's finalize), in beam order. */
+RVB_API int rvb_ctc_prefix_beam_search_biased(const float* d_topk_val, const int* d_topk_idx, int k,
+                                              const int* h_enc_lens, int B, int Tp, int beam, int blank_id, int max_len,
+                                              int* h_tokens, int* h_times, int* h_lens, double* h_scores, int* h_nhyp,
+                                              rvb_context_graph* graph, void* stream);
+
 /* Teacher-forced (bi-)decoder over the n-best.  h_hyp_tokens (B, N, max_len), h_hyp_lens (B, N) (a negative length
  * marks an absent hypothesis).  h_l2r (B, N, max_len + 1): [j] = log p(w_j | ...) for j < U, [U] = log p(eos);
  * h_r2l likewise for the right-to-left decoder with [j] = r_logp[U-1-j][w_j], [U] = r_logp[U][eos]
@@ -170,6 +192,11 @@ RVB_API int rvb_beam_search_rescoring(rvb_model* m, const float* d_topk_val, con
  *                         hypothesis order and frees the ticket. */
 RVB_API int rvb_search_submit(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k, const float* d_enc_out,
                               const int* h_enc_lens, int B, int Tp, int beam, int blank_id, void* stream);
+/* rvb_search_submit with context biasing (see rvb_ctc_prefix_beam_search_biased); the rest of the ticket is unchanged.
+ * The graph must not be destroyed before the ticket is collected or released. */
+RVB_API int rvb_search_submit_biased(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k,
+                                     const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int beam, int blank_id,
+                                     rvb_context_graph* graph, void* stream);
 RVB_API int rvb_rescoring_submit(rvb_model* m, int ticket, const float* h_cat_embs, int n_cat, float reverse_weight, int cap,
                                  int run_decoder, int* h_tokens, int* h_times, float* h_l2r, float* h_r2l,
                                  int* out_max_len, void* stream);

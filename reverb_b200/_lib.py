@@ -67,6 +67,11 @@ SIGNATURES = {
     "rvb_beam_search_rescoring": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _f, _i, _vp, _vp, _vp, _vp, _vp,
                                        _vp, _vp, _vp, _vp]),
     "rvb_search_submit": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "rvb_search_submit_biased": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "rvb_context_graph_create": (_vp, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i]),
+    "rvb_context_graph_destroy": (None, [_vp]),
+    "rvb_ctc_prefix_beam_search_biased": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               _vp]),
     "rvb_rescoring_submit": (_i, [_vp, _i, _vp, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rvb_rescoring_collect": (_i, [_vp, _i, _vp, _vp, _vp]),
     "rvb_ticket_release": (_i, [_vp, _i]),

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from .engine import Engine, check_beam_size
-from .search import (DecodeResult, attention_beam_search, ctc_prefix_beam_search_biased, greedy_results,
+from .search import (DecodeResult, attention_beam_search, greedy_results,
                      joint_decoding_results, prefix_beam_results, rescoring_pick, rescoring_pick_batch,
                      time_sync_joint_search)
 
@@ -160,20 +160,11 @@ class ASRModel:
                                                              pre_beam, beam_size, ctc_weight, length_penalty, cat_embs)
             if need_beam and k != beam_size:                  # the searches below expect exactly beam_size candidates
                 topk_val, topk_idx = topk_val[:, :, :beam_size].contiguous(), topk_idx[:, :, :beam_size].contiguous()
-        if need_beam and context_graph is not None:
-            # context biasing (search.py:124-248 with a ContextGraph): the per-prefix automaton state makes this a host
-            # search over the GPU's per-frame top-k, like the reference's; the n-best then goes through the ordinary
-            # rescoring decoder.  Not a throughput path (the reverb CLI never builds a graph, cli/reverb.py:227).
-            prefix = ctc_prefix_beam_search_biased(topk_val.cpu().numpy(), topk_idx.cpu().numpy(), encoder_lens, beam_size,
-                                                   context_graph, blank_id)
-            if "ctc_prefix_beam_search" in methods:
-                results["ctc_prefix_beam_search"] = prefix
-            if "attention_rescoring" in methods:
-                results["attention_rescoring"] = self.attention_rescoring(prefix, encoder_out, encoder_lens, ctc_weight,
-                                                                          reverse_weight, cat_embs)
-        elif need_beam:
-            # the n-best stays on the device between the search and the decoder (native ticket, include/rvb_b200.h)
-            st["ticket"] = self.engine.search_submit(topk_val, topk_idx, encoder_out, encoder_lens, beam_size, blank_id)
+        if need_beam:
+            # the n-best stays on the device between the search and the decoder (native ticket, include/rvb_b200.h);
+            # with a context graph the search is the biased instantiation of the same kernel (search.py:124-248)
+            st["ticket"] = self.engine.search_submit(topk_val, topk_idx, encoder_out, encoder_lens, beam_size, blank_id,
+                                                     context=context_graph)
         return st
 
     def _joint_decoding(self, encoder_out, encoder_lens, topk_val, topk_idx, logp_full, pre_beam, beam_size,

@@ -11,21 +11,25 @@ a phrase that ends on an already existing node does not mark it as a phrase end 
 Representation: states are plain integers (0 = root) indexing parallel lists — `children[s]` (token -> state),
 `fail[s]`, `bonus[s]`, `emit[s]` — instead of linked node objects; `ASRModel.decode(context_graph=...)` and
 `reverb_b200.search.ctc_prefix_beam_search_biased` only use `root`, `forward_one_step` and `finalize`, so the
-reference's own `ContextGraph` object can be passed as well.  The reverb CLI never builds a graph (cli/reverb.py:227).
+reference's own `ContextGraph` object can be passed as well.  The GPU search takes either form through `device_tables`,
+which compiles the automaton to the flat tables the device holds (csrc/context.cu).
 """
 from __future__ import annotations
 
+import os
 import re
 from typing import Dict, Iterable, List, Optional, Sequence, Tuple
+
+import numpy as np
 
 _CJK = re.compile(r"([一-鿿])")
 
 
-def tokenize(context_list_path: str, symbol_table: Dict[str, int], bpe_model: Optional[str] = None) -> List[List[int]]:
-    """One biasing phrase per line -> token ids.  With a sentencepiece model: upper-cased text, CJK characters on their
-    own, everything else through `encode_as_pieces` (text/tokenize_utils.py:19-60); without: one symbol per character,
-    space written as the word-boundary mark.  Symbols missing from the table become <unk> if the table has it and are
-    dropped otherwise."""
+def tokenize(context_list_path, symbol_table: Dict[str, int], bpe_model: Optional[str] = None) -> List[List[int]]:
+    """One biasing phrase per line -> token ids.  `context_list_path` is a file path or the lines themselves (any
+    iterable of strings).  With a sentencepiece model: upper-cased text, CJK characters on their own, everything else
+    through `encode_as_pieces` (text/tokenize_utils.py:19-60); without: one symbol per character, space written as the
+    word-boundary mark.  Symbols missing from the table become <unk> if the table has it and are dropped otherwise."""
     encode = None
     if bpe_model is not None:
         import sentencepiece as spm
@@ -39,14 +43,16 @@ def tokenize(context_list_path: str, symbol_table: Dict[str, int], bpe_model: Op
                     pieces.extend([part] if _CJK.fullmatch(part) else sp.encode_as_pieces(part))
             return pieces
     unk = symbol_table.get("<unk>")
-    phrases: List[List[int]] = []
-    with open(context_list_path, "r") as f:
-        for line in f:
-            text = line.strip()
-            symbols = encode(text) if encode else [("▁" if ch == " " else ch) for ch in text]
-            ids = [symbol_table.get(sym, unk) for sym in symbols]
-            phrases.append([i for i in ids if i is not None])
-    return phrases
+
+    def phrase(line: str) -> List[int]:
+        text = line.strip()
+        symbols = encode(text) if encode else [("▁" if ch == " " else ch) for ch in text]
+        ids = [symbol_table.get(sym, unk) for sym in symbols]
+        return [i for i in ids if i is not None]
+    if isinstance(context_list_path, (str, os.PathLike)):
+        with open(context_list_path, "r") as f:
+            return [phrase(line) for line in f]
+    return [phrase(line) for line in context_list_path]
 
 
 class ContextGraph:
@@ -134,3 +140,92 @@ class ContextGraph:
     def finalize(self, state: int) -> Tuple[float, int]:
         """Take back the bonus of a match that did not complete; the next state is the root."""
         return -self.bonus[state], 0
+
+
+# -- device tables ----------------------------------------------------------------------------------------------------
+def _linked_states(root) -> list:
+    """The states of a linked-node graph (the reference's `ContextState`: `.next`, `.fail`, `.node_score`,
+    `.output_score`, `.token_score`) indexed by their `id` when the ids number the states 0..n-1 with the root at 0,
+    else in breadth-first order from the root."""
+    order, seen, head = [root], {id(root)}, 0
+    while head < len(order):
+        for child in order[head].next.values():
+            if id(child) not in seen:
+                seen.add(id(child))
+                order.append(child)
+        head += 1
+    ids = [getattr(s, "id", None) for s in order]
+    if all(isinstance(i, int) for i in ids) and sorted(ids) == list(range(len(order))) and ids[0] == 0:
+        states = [None] * len(order)
+        for s in order:
+            states[s.id] = s
+        return states
+    return order
+
+
+def device_tables(graph) -> Dict[str, np.ndarray]:
+    """Compile a context graph — this module's `ContextGraph` or the reference's linked `ContextState` graph — to the
+    flat tables the GPU search reads (include/rvb_b200.h rvb_context_graph_create): state 0 = root; `off` (n + 1) /
+    `tok` / `dst` the children in CSR by state, sorted by token; `fail` (n); `bonus` (node_score), `emit`
+    (output_score) and `token_score` as float64, the host values as they are."""
+    if isinstance(graph.root, (int, np.integer)):
+        n = len(graph.children)
+        children = [sorted(c.items()) for c in graph.children]
+        fail = list(graph.fail)
+        bonus, emit = list(graph.bonus), list(graph.emit)
+        # forward_one_step scores a matched child with the graph's context_score (the reference: node.token_score)
+        token_score = [0.0] + [float(graph.context_score)] * (n - 1)
+    else:
+        states = _linked_states(graph.root)
+        index = {id(s): i for i, s in enumerate(states)}
+        n = len(states)
+        children = [sorted((tok, index[id(c)]) for tok, c in s.next.items()) for s in states]
+        fail = [index[id(s.fail)] if s.fail is not None else 0 for s in states]
+        bonus = [s.node_score for s in states]
+        emit = [s.output_score for s in states]
+        token_score = [s.token_score for s in states]
+    off = np.zeros(n + 1, dtype=np.int64)
+    off[1:] = np.cumsum([len(c) for c in children])
+    tok = np.fromiter((t for c in children for t, _ in c), dtype=np.int64, count=int(off[-1]))
+    dst = np.fromiter((d for c in children for _, d in c), dtype=np.int64, count=int(off[-1]))
+    return {"off": off, "tok": tok, "dst": dst, "fail": np.asarray(fail, dtype=np.int64),
+            "bonus": np.asarray(bonus, dtype=np.float64), "emit": np.asarray(emit, dtype=np.float64),
+            "token_score": np.asarray(token_score, dtype=np.float64)}
+
+
+def check_device_tables(t: Dict[str, np.ndarray], vocab: int, blank_id: int) -> None:
+    """ValueError unless `t` (device_tables) is a graph the GPU search can walk: at most 2^31 - 1 states, a trie
+    reachable from the root, tokens in [0, vocab) and not the blank, fail links to strictly shallower states (every fail
+    walk ends at the root), finite scores.  The native upload repeats these checks."""
+    n = int(t["fail"].shape[0])
+    if not 1 <= n <= np.iinfo(np.int32).max:
+        raise ValueError(f"context graph: {n} states do not fit int32 indices")
+    off, tok, dst, fail = t["off"], t["tok"], t["dst"], t["fail"]
+    if off.shape[0] != n + 1 or off[0] != 0 or off[-1] != n - 1 or tok.shape[0] != n - 1 or dst.shape[0] != n - 1 \
+            or np.any(np.diff(off) < 0):
+        raise ValueError("context graph: the child tables are not a trie over the states")
+    for name in ("bonus", "emit", "token_score"):
+        if t[name].shape[0] != n or not np.all(np.isfinite(t[name])):
+            raise ValueError(f"context graph: {name} must hold one finite value per state")
+    bad = (tok < 0) | (tok >= vocab) | (tok == blank_id)
+    if np.any(bad):
+        raise ValueError(f"context graph: token {int(tok[np.argmax(bad)])} is not a non-blank id of the "
+                         f"{vocab}-entry vocabulary (blank {blank_id})")
+    depth = np.full(n, -1, dtype=np.int64)
+    depth[0] = 0
+    order, head = [0], 0
+    while head < len(order):
+        s = order[head]
+        head += 1
+        lo, hi = int(off[s]), int(off[s + 1])
+        if np.any(np.diff(tok[lo:hi]) <= 0):
+            raise ValueError(f"context graph: children of state {s} are not sorted by token")
+        for c in dst[lo:hi].tolist():
+            if not 0 < c < n or depth[c] >= 0:
+                raise ValueError(f"context graph: state {c} is out of range or has two parents")
+            depth[c] = depth[s] + 1
+            order.append(c)
+    if len(order) != n:
+        raise ValueError(f"context graph: {n - len(order)} states are unreachable from the root")
+    if fail[0] != 0 or np.any((fail < 0) | (fail >= n)) or np.any(depth[fail[1:]] >= depth[1:]):
+        raise ValueError("context graph: a fail link does not lead toward the root")

@@ -7,7 +7,8 @@
 //                     utils/ctc_utils.py:22-32).
 //   ctc_prefix_beam : CTC prefix beam search with the reference's exact update rules, float64 score arithmetic and
 //                     Viterbi time tracking (search.py:124-248, utils/common.py:355-363) — one warp per utterance,
-//                     prefixes as canonical trie nodes, times as persistent linked lists.
+//                     prefixes as canonical trie nodes, times as persistent linked lists.  The biased instantiation
+//                     adds the context-graph state of every prefix (the `context_graph` branches of the same lines).
 //   logsoftmax_gather : rescoring decoder output -> log-probs of the hypothesis tokens only (search.py:413-436).
 #include <math.h>
 
@@ -269,6 +270,55 @@ constexpr int PB_THREADS = 128;
 constexpr int PB_EXT_THREADS = PB_THREADS - 32;  // warps 0..2: extension candidates; last warp: stay slots
 constexpr int PB_KEY_NONE = 0x7fffffff;
 
+// Context biasing (biased instantiation only).  A prefix's context state and score depend on its token sequence alone
+// (blank and repeat keep them, an extension takes one automaton step from its parent), so they travel with the beam
+// entry and the reference's "first writer sets has_context" rule never has to be replayed.  These arrays live in dynamic
+// shared memory in front of the trie, so the plain search's static layout is untouched.
+struct PBCtx {
+  double csc[2][PB_MAXBEAM];       // context score of every beam entry (both beam buffers)
+  double slot_csc[PB_MAXSLOTS];    // context score of every slot of the frame
+  double slot_tot[PB_MAXSLOTS];    // rank key of every slot: score() + context score (PrefixScore.total_score)
+  int cst[2][PB_MAXBEAM];          // context state of every beam entry
+  int slot_cst[PB_MAXSLOTS];
+};
+static_assert(sizeof(PBCtx) % 16 == 0, "the trie follows PBCtx in dynamic shared memory");
+
+// One automaton step (utils/context_graph.py forward_one_step / fail walk; context_graph.py of this package): the
+// child of `s` on `u` if there is one (token_score), else the fail walk from fail[s] that stops at the root, then the
+// root's child if the walk ended there (bonus difference); plus the output bonus of the state reached.
+__device__ __forceinline__ int ctx_child(const ContextGraphView& g, int s, int u) {
+  if (s == 0) return u < g.vocab ? __ldg(g.root_next + u) : -1;
+  int lo = __ldg(g.off + s);
+  const int end = __ldg(g.off + s + 1);
+  int hi = end;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(g.tok + mid) < u) lo = mid + 1;
+    else hi = mid;
+  }
+  return (lo < end && __ldg(g.tok + lo) == u) ? __ldg(g.dst + lo) : -1;
+}
+__device__ __forceinline__ double ctx_step(const ContextGraphView& g, int s, int u, int* next) {
+  int n = ctx_child(g, s, u);
+  double gained;
+  if (n >= 0) {
+    gained = __ldg(g.token_score + n);
+  } else {
+    int f = __ldg(g.fail + s);
+    while ((n = ctx_child(g, f, u)) < 0) {
+      f = __ldg(g.fail + f);
+      if (f == 0) {
+        n = ctx_child(g, 0, u);
+        break;
+      }
+    }
+    if (n < 0) n = f;
+    gained = __ldg(g.bonus + n) - __ldg(g.bonus + s);
+  }
+  *next = n;
+  return gained + __ldg(g.emit + n);
+}
+
 // The beam entering a frame: score()/viterbi_score()/times() of every prefix are derived when the entry is created.
 struct PBBeam {
   double s[PB_MAXBEAM], ns[PB_MAXBEAM], vs[PB_MAXBEAM], vns[PB_MAXBEAM], score[PB_MAXBEAM], vit[PB_MAXBEAM];
@@ -286,16 +336,22 @@ struct PBBeam {
 //       the OTHER beam buffer: canonical trie node (find-or-create in a shared-memory hash), times list nodes
 // The next frame's top-k is prefetched into registers during P1.  Prefix identity = canonical trie node id, so the
 // dict-merge semantics of the reference hold exactly.
+// kBiased: context biasing with graph `cg` — P3 ranks by score() + context score, the recursion itself still uses
+// score() / viterbi_score() alone, and the emitted score is score() - bonus[state] (finalize, search.py:226-233).
+// The plain instantiation ignores `cg` and compiles to the code it had before biasing existed.
+template <bool kBiased>
 __global__ void __launch_bounds__(PB_THREADS)
 ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict__ topk_idx, int k,
                        const int* __restrict__ lens, int T, int beam, int blank, int* __restrict__ workspace,
                        int trie_in_smem, int max_len, int* __restrict__ out_tokens, int* __restrict__ out_times,
-                       int* __restrict__ out_lens, double* __restrict__ out_scores, int* __restrict__ out_nhyp) {
+                       int* __restrict__ out_lens, double* __restrict__ out_scores, int* __restrict__ out_nhyp,
+                       ContextGraphView cg) {
   extern __shared__ int pb_dyn[];
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const PBLayout L = pb_layout(T, beam);
   int* ws = workspace + (size_t)b * L.per_utt_ints;
-  int* trie_parent = trie_in_smem ? pb_dyn : ws;
+  PBCtx* cx = reinterpret_cast<PBCtx*>(pb_dyn);
+  int* trie_parent = trie_in_smem ? (kBiased ? pb_dyn + sizeof(PBCtx) / sizeof(int) : pb_dyn) : ws;
   int* trie_tok = trie_parent + L.pool_cap;
   int* hash = trie_parent + 2 * L.pool_cap;  // -1 = empty
   int* times_parent = ws + 2 * L.pool_cap + L.hash_cap;
@@ -333,6 +389,10 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
     C.times[0] = -1;
     C.last[0] = -1;
     C.par[0] = -1;
+    if constexpr (kBiased) {
+      cx->cst[0][0] = 0;  // the root
+      cx->csc[0][0] = 0.0;
+    }
   }
   if (tid < kk && len > 0) {
     s_tv[0][tid] = (double)topk_val[((long long)b * T) * k + tid];
@@ -437,6 +497,12 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
           slot_key[j] = kmin;
           slot_score[j] = (kmin == PB_KEY_NONE) ? PB_NEG_INF : log_add2(s_other, ns_new);
           mylive = (kmin != PB_KEY_NONE);
+          if constexpr (kBiased) {  // the prefix is unchanged: so are its context state and score
+            const double csc = cx->csc[cur][j];
+            cx->slot_cst[j] = cx->cst[cur][j];
+            cx->slot_csc[j] = csc;
+            cx->slot_tot[j] = (kmin == PB_KEY_NONE) ? PB_NEG_INF : slot_score[j] + csc;
+          }
         }
       }
     } else {
@@ -446,7 +512,7 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
         const int u = ti[ui];
         const double p = tv[ui];
         int key = PB_KEY_NONE;
-        double sc = PB_NEG_INF;
+        double sc = PB_NEG_INF, tot = PB_NEG_INF;
         if (u != blank) {
           const int node_i = C.node[i];
           bool collide = false;
@@ -476,10 +542,19 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
             key = 2 * c + 1;
             sc = add + p;  // score() = log_add([-inf, ns]) = ns
             ++mylive;
+            if constexpr (kBiased) {  // one automaton step from the parent's state
+              int nst;
+              const double step = ctx_step(cg, cx->cst[cur][i], u, &nst);
+              const double csc = cx->csc[cur][i] + step;
+              cx->slot_cst[nb + c] = nst;
+              cx->slot_csc[nb + c] = csc;
+              tot = sc + csc;
+            }
           }
         }
         slot_key[nb + c] = key;
         slot_score[nb + c] = sc;
+        if constexpr (kBiased) cx->slot_tot[nb + c] = tot;
       }
     }
     mylive = __reduce_add_sync(0xffffffffu, mylive);
@@ -492,16 +567,19 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
       s_tv[cur ^ 1][tid] = (double)pre_v;
       s_ti[cur ^ 1][tid] = pre_i;
     }
+    // rank key: score(), or score() + context score when biased
+    const double* rank_key = slot_score;
+    if constexpr (kBiased) rank_key = cx->slot_tot;
     for (int a = tid; a < nslots; a += PB_THREADS) {
       const int key = slot_key[a];
       if (key == PB_KEY_NONE) continue;
-      const double sc = slot_score[a];
+      const double sc = rank_key[a];
       // dead slots carry (score -inf, key INT_MAX): they never count, so the loop needs no liveness branch
       // four independent counters: the compare -> add chains overlap instead of serialising on one register
       int r0 = 0, r1 = 0, r2 = 0, r3 = 0;
       int o = 0;
       for (; o + 4 <= nslots; o += 4) {
-        const double s0 = slot_score[o], s1 = slot_score[o + 1], s2 = slot_score[o + 2], s3 = slot_score[o + 3];
+        const double s0 = rank_key[o], s1 = rank_key[o + 1], s2 = rank_key[o + 2], s3 = rank_key[o + 3];
         const int k0 = slot_key[o], k1 = slot_key[o + 1], k2 = slot_key[o + 2], k3 = slot_key[o + 3];
         r0 += (int)((s0 > sc) | ((s0 == sc) & (k0 < key)));
         r1 += (int)((s1 > sc) | ((s1 == sc) & (k1 < key)));
@@ -509,7 +587,7 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
         r3 += (int)((s3 > sc) | ((s3 == sc) & (k3 < key)));
       }
       for (; o < nslots; ++o) {
-        const double so = slot_score[o];
+        const double so = rank_key[o];
         r0 += (int)((so > sc) | ((so == sc) & (slot_key[o] < key)));
       }
       const int rank = (r0 + r1) + (r2 + r3);
@@ -560,7 +638,7 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
       N.ns[rank] = s.ns;
       N.vs[rank] = s.vs;
       N.vns[rank] = s.vns;
-      N.score[rank] = sc;
+      N.score[rank] = kBiased ? slot_score[a] : sc;
       N.vit[rank] = sb ? s.vs : s.vns;
       N.ts[rank] = s.times_s;
       N.tns[rank] = tns;
@@ -568,6 +646,10 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
       N.times[rank] = sb ? s.times_s : tns;
       N.last[rank] = (s.tok < 0) ? C.last[s.src] : s.tok;
       N.par[rank] = (s.tok < 0) ? C.par[s.src] : C.node[s.src];
+      if constexpr (kBiased) {
+        cx->cst[cur ^ 1][rank] = cx->slot_cst[a];
+        cx->csc[cur ^ 1][rank] = cx->slot_csc[a];
+      }
     }
     nb = nnew;
     __syncthreads();
@@ -597,13 +679,20 @@ ctc_prefix_beam_kernel(const float* __restrict__ topk_val, const int* __restrict
     }
     out_lens[(b * beam + r) * 2 + 0] = n;
     out_lens[(b * beam + r) * 2 + 1] = nt;
-    out_scores[b * beam + r] = F.score[r];
+    if constexpr (kBiased) {
+      // finalize: the context score becomes -bonus[state] (an unfinished match is taken back); no re-sort
+      out_scores[b * beam + r] = F.score[r] + (-__ldg(cg.bonus + cx->cst[len & 1][r]));
+    } else {
+      out_scores[b * beam + r] = F.score[r];
+    }
   }
 }
 
-int launch_ctc_prefix_beam(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T, int beam,
-                           int blank, void* workspace, size_t workspace_bytes, int max_len, int* out_tokens,
-                           int* out_times, int* out_lens, double* out_scores, int* out_nhyp, cudaStream_t stream) {
+template <bool kBiased>
+static int launch_prefix_beam(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T, int beam,
+                              int blank, void* workspace, size_t workspace_bytes, int max_len, int* out_tokens,
+                              int* out_times, int* out_lens, double* out_scores, int* out_nhyp,
+                              const ContextGraphView& cg, cudaStream_t stream) {
   RVB_REQUIRE(beam >= 1 && beam <= PB_MAXBEAM, "prefix beam: beam_size=%d unsupported (1..%d)", beam, PB_MAXBEAM);
   RVB_REQUIRE(k >= beam, "prefix beam: need top-k with k >= beam (k=%d beam=%d)", k, beam);
   const size_t need = prefix_beam_workspace_bytes(B, T, beam);
@@ -613,15 +702,32 @@ int launch_ctc_prefix_beam(const float* topk_val, const int* topk_idx, int k, co
   const size_t trie_bytes = ((size_t)2 * L.pool_cap + L.hash_cap) * sizeof(int);
   const int trie_in_smem = trie_bytes <= 150 * 1024;
   if (!trie_in_smem) RVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0xFF, need, stream));  // hash tables = -1
-  const size_t dyn = trie_in_smem ? trie_bytes : 0;
+  const size_t dyn = (trie_in_smem ? trie_bytes : 0) + (kBiased ? sizeof(PBCtx) : 0);
   static DynSmemOptIn optin;
-  if (optin.ensure(ctc_prefix_beam_kernel, dyn)) return -1;
-  ctc_prefix_beam_kernel<<<B, PB_THREADS, dyn, stream>>>(topk_val, topk_idx, k, lens, T, beam, blank,
-                                                        reinterpret_cast<int*>(workspace), trie_in_smem, max_len,
-                                                        out_tokens, out_times, out_lens, out_scores, out_nhyp);
+  if (optin.ensure(ctc_prefix_beam_kernel<kBiased>, dyn)) return -1;
+  ctc_prefix_beam_kernel<kBiased><<<B, PB_THREADS, dyn, stream>>>(topk_val, topk_idx, k, lens, T, beam, blank,
+                                                                 reinterpret_cast<int*>(workspace), trie_in_smem,
+                                                                 max_len, out_tokens, out_times, out_lens, out_scores,
+                                                                 out_nhyp, cg);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
   return 0;
+}
+
+int launch_ctc_prefix_beam(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T, int beam,
+                           int blank, void* workspace, size_t workspace_bytes, int max_len, int* out_tokens,
+                           int* out_times, int* out_lens, double* out_scores, int* out_nhyp, cudaStream_t stream) {
+  return launch_prefix_beam<false>(topk_val, topk_idx, k, lens, B, T, beam, blank, workspace, workspace_bytes, max_len,
+                                   out_tokens, out_times, out_lens, out_scores, out_nhyp, ContextGraphView{}, stream);
+}
+
+int launch_ctc_prefix_beam_biased(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T,
+                                  int beam, int blank, void* workspace, size_t workspace_bytes, int max_len,
+                                  int* out_tokens, int* out_times, int* out_lens, double* out_scores, int* out_nhyp,
+                                  const ContextGraphView& graph, cudaStream_t stream) {
+  RVB_REQUIRE(graph.off && graph.root_next && graph.bonus, "prefix beam: context graph not uploaded");
+  return launch_prefix_beam<true>(topk_val, topk_idx, k, lens, B, T, beam, blank, workspace, workspace_bytes, max_len,
+                                  out_tokens, out_times, out_lens, out_scores, out_nhyp, graph, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

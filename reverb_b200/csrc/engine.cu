@@ -1587,9 +1587,10 @@ int search_side_stream(rvb_model* m, cudaStream_t* out) {
   return 0;
 }
 
+// graph != nullptr: the biased search (context biasing with that graph)
 static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val, const int* d_topk_idx, int k,
                          const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int beam, int blank_id,
-                         DevBuf& ws, cudaStream_t stream) {
+                         ::rvb_context_graph* graph, DevBuf& ws, cudaStream_t stream) {
   const int S = B * beam, dev_len = Tp;  // a prefix never has more tokens than frames
   t.B = B;
   t.Tp = Tp;
@@ -1634,9 +1635,17 @@ static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val,
     RVB_CHECK_CUDA(cudaStreamWaitEvent(ss, m->ev_topk, 0));
   }
   RVB_CHECK_CUDA(cudaMemcpyAsync(t.d_lens(), hp_elen, sizeof(int) * B, cudaMemcpyHostToDevice, ss));
-  if (launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, t.d_lens(), B, Tp, beam, blank_id, ws.p, ws.cap, dev_len,
-                             t.d_tok(), t.d_tim(), t.d_olen(), t.d_sc(), t.d_nhyp(), ss))
-    return -1;
+  if (graph == nullptr) {
+    if (launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, t.d_lens(), B, Tp, beam, blank_id, ws.p, ws.cap, dev_len,
+                               t.d_tok(), t.d_tim(), t.d_olen(), t.d_sc(), t.d_nhyp(), ss))
+      return -1;
+  } else {
+    if (launch_ctc_prefix_beam_biased(d_topk_val, d_topk_idx, k, t.d_lens(), B, Tp, beam, blank_id, ws.p, ws.cap,
+                                      dev_len, t.d_tok(), t.d_tim(), t.d_olen(), t.d_sc(), t.d_nhyp(),
+                                      *context_graph_view(graph), ss) ||
+        context_graph_note_use(graph, ss))
+      return -1;
+  }
   RVB_CHECK_CUDA(cudaMemcpyAsync(hp_small, t.d_olen(), t.small_bytes, cudaMemcpyDeviceToHost, ss));
   for (int dir = 0; dir < ndir; ++dir) {
     TrieView v = t.trie_view(dir);
@@ -1984,10 +1993,9 @@ RVB_API int rvb_ctc_greedy_search(const int* d_topk_idx, int k, const int* h_enc
   return 0;
 }
 
-RVB_API int rvb_ctc_prefix_beam_search(const float* d_topk_val, const int* d_topk_idx, int k, const int* h_enc_lens, int B,
-                               int Tp, int beam, int blank_id, int max_len, int* h_tokens, int* h_times, int* h_lens,
-                               double* h_scores, int* h_nhyp, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+static int prefix_beam_search(const float* d_topk_val, const int* d_topk_idx, int k, const int* h_enc_lens, int B, int Tp,
+                              int beam, int blank_id, int max_len, int* h_tokens, int* h_times, int* h_lens,
+                              double* h_scores, int* h_nhyp, rvb_context_graph* graph, cudaStream_t stream) {
   RVB_REQUIRE(d_topk_val && d_topk_idx && h_enc_lens && h_tokens && h_times && h_lens && h_scores && h_nhyp && B > 0 &&
                   Tp > 0 && max_len > 0,
               "rvb_ctc_prefix_beam_search: bad arguments");
@@ -2008,9 +2016,17 @@ RVB_API int rvb_ctc_prefix_beam_search(const float* d_topk_val, const int* d_top
   memcpy(hp, h_enc_lens, sizeof(int) * B);
   RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, hp, sizeof(int) * B, cudaMemcpyHostToDevice, stream));
   RVB_CHECK_CUDA(cudaMemsetAsync(d_tok, 0, (ints - B) * sizeof(int), stream));
-  if (rvb::launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, d_lens, B, Tp, beam, blank_id, g_search_ws.p, g_search_ws.cap,
-                                  max_len, d_tok, d_tim, d_olen, d_sc, d_nhyp, stream))
-    return -1;
+  if (graph == nullptr) {
+    if (rvb::launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, d_lens, B, Tp, beam, blank_id, g_search_ws.p,
+                                    g_search_ws.cap, max_len, d_tok, d_tim, d_olen, d_sc, d_nhyp, stream))
+      return -1;
+  } else {
+    if (rvb::launch_ctc_prefix_beam_biased(d_topk_val, d_topk_idx, k, d_lens, B, Tp, beam, blank_id, g_search_ws.p,
+                                           g_search_ws.cap, max_len, d_tok, d_tim, d_olen, d_sc, d_nhyp,
+                                           *rvb::context_graph_view(graph), stream) ||
+        rvb::context_graph_note_use(graph, stream))
+      return -1;
+  }
   RVB_CHECK_CUDA(cudaMemcpyAsync(hp, g_search_out.p, out_bytes, cudaMemcpyDeviceToHost, stream));
   RVB_CHECK_CUDA(cudaStreamSynchronize(stream));
   memcpy(h_tokens, hp + B, n_tok * sizeof(int));
@@ -2025,13 +2041,30 @@ RVB_API int rvb_ctc_prefix_beam_search(const float* d_topk_val, const int* d_top
   return 0;
 }
 
+RVB_API int rvb_ctc_prefix_beam_search(const float* d_topk_val, const int* d_topk_idx, int k, const int* h_enc_lens, int B,
+                               int Tp, int beam, int blank_id, int max_len, int* h_tokens, int* h_times, int* h_lens,
+                               double* h_scores, int* h_nhyp, void* stream) {
+  return prefix_beam_search(d_topk_val, d_topk_idx, k, h_enc_lens, B, Tp, beam, blank_id, max_len, h_tokens, h_times,
+                            h_lens, h_scores, h_nhyp, nullptr, (cudaStream_t)stream);
+}
+
+RVB_API int rvb_ctc_prefix_beam_search_biased(const float* d_topk_val, const int* d_topk_idx, int k,
+                                              const int* h_enc_lens, int B, int Tp, int beam, int blank_id, int max_len,
+                                              int* h_tokens, int* h_times, int* h_lens, double* h_scores, int* h_nhyp,
+                                              rvb_context_graph* graph, void* stream) {
+  RVB_REQUIRE(graph != nullptr, "rvb_ctc_prefix_beam_search_biased: no context graph");
+  return prefix_beam_search(d_topk_val, d_topk_idx, k, h_enc_lens, B, Tp, beam, blank_id, max_len, h_tokens, h_times,
+                            h_lens, h_scores, h_nhyp, graph, (cudaStream_t)stream);
+}
+
 static rvb::SearchTicket* ticket_of(rvb_model* m, int id) {
   if (m == nullptr || m->tickets == nullptr || id < 0 || id >= rvb_model::kTickets) return nullptr;
   return &m->tickets[id];
 }
 
-RVB_API int rvb_search_submit(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k, const float* d_enc_out,
-                              const int* h_enc_lens, int B, int Tp, int beam, int blank_id, void* stream) {
+static int search_submit_any(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k, const float* d_enc_out,
+                             const int* h_enc_lens, int B, int Tp, int beam, int blank_id, rvb_context_graph* graph,
+                             void* stream) {
   RVB_REQUIRE(m && d_topk_val && d_topk_idx && d_enc_out && h_enc_lens && B > 0 && Tp > 0 && beam > 0,
               "rvb_search_submit: bad arguments");
   if (m->tickets == nullptr) m->tickets = new rvb::SearchTicket[rvb_model::kTickets];
@@ -2044,11 +2077,23 @@ RVB_API int rvb_search_submit(rvb_model* m, const float* d_topk_val, const int* 
   RVB_REQUIRE(id >= 0, "rvb_search_submit: all %d tickets of this plan are in flight (collect one first)",
               rvb_model::kTickets);
   if (rvb::search_submit(m, m->tickets[id], d_topk_val, d_topk_idx, k, d_enc_out, h_enc_lens, B, Tp, beam, blank_id,
-                         g_search_ws, (cudaStream_t)stream)) {
+                         graph, g_search_ws, (cudaStream_t)stream)) {
     m->tickets[id].state = 0;
     return -1;
   }
   return id;
+}
+
+RVB_API int rvb_search_submit(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k, const float* d_enc_out,
+                              const int* h_enc_lens, int B, int Tp, int beam, int blank_id, void* stream) {
+  return search_submit_any(m, d_topk_val, d_topk_idx, k, d_enc_out, h_enc_lens, B, Tp, beam, blank_id, nullptr, stream);
+}
+
+RVB_API int rvb_search_submit_biased(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k,
+                                     const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int beam, int blank_id,
+                                     rvb_context_graph* graph, void* stream) {
+  RVB_REQUIRE(graph != nullptr, "rvb_search_submit_biased: no context graph");
+  return search_submit_any(m, d_topk_val, d_topk_idx, k, d_enc_out, h_enc_lens, B, Tp, beam, blank_id, graph, stream);
 }
 
 RVB_API int rvb_rescoring_submit(rvb_model* m, int ticket, const float* h_cat_embs, int n_cat, float reverse_weight, int cap,

@@ -4,6 +4,7 @@
 #include "common.cuh"
 
 struct rvb_model;
+struct rvb_context_graph;
 
 namespace rvb {
 
@@ -232,6 +233,29 @@ size_t prefix_beam_workspace_bytes(int B, int T, int beam);
 int launch_ctc_prefix_beam(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T, int beam,
                            int blank, void* workspace, size_t workspace_bytes, int max_len, int* out_tokens,
                            int* out_times, int* out_lens, double* out_scores, int* out_nhyp, cudaStream_t stream);
+// Context graph in read-only device memory (context.cu): children in CSR by state with token-sorted child lists,
+// the root's children also as a dense token -> child table (-1 = none), fail links, and the float64 tables of
+// utils/context_graph.py (node_score = bonus, output_score = emit, token_score).  State 0 is the root.
+struct ContextGraphView {
+  const int* off = nullptr;        // n_nodes + 1
+  const int* tok = nullptr;        // n_edges, sorted within a state
+  const int* dst = nullptr;        // n_edges
+  const int* fail = nullptr;       // n_nodes
+  const int* root_next = nullptr;  // vocab
+  const double* bonus = nullptr;
+  const double* emit = nullptr;
+  const double* token_score = nullptr;
+  int n_nodes = 0, vocab = 0;
+};
+// the same search with context biasing (the `context_graph` branches of search.py:124-248)
+int launch_ctc_prefix_beam_biased(const float* topk_val, const int* topk_idx, int k, const int* lens, int B, int T,
+                                  int beam, int blank, void* workspace, size_t workspace_bytes, int max_len,
+                                  int* out_tokens, int* out_times, int* out_lens, double* out_scores, int* out_nhyp,
+                                  const ContextGraphView& graph, cudaStream_t stream);
+// the device tables of a graph handle (context.cu), and the bookkeeping that lets rvb_context_graph_destroy wait for
+// searches enqueued with it: call after enqueueing such a search on `stream`
+const ContextGraphView* context_graph_view(const ::rvb_context_graph* g);
+int context_graph_note_use(::rvb_context_graph* g, cudaStream_t stream);
 
 // ------------------------------------------------------------------ rescoring (ctc.cu)
 // per row r: lse = logsumexp(logits[r, :V]); out[r, j] = logits[r, gather_idx[r*G + j]] - lse  (idx < 0 -> 0)

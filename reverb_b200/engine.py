@@ -5,6 +5,7 @@ FLOP of the hot path runs in the hand-written sm_90a kernels behind the C ABI.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -86,6 +87,42 @@ def model_config_from_yaml(configs: Dict, vocab: int, precision: str = "bf16") -
     cfg.eos_id = int(st.get("<eos>", vocab - 1))
     cfg.precision = PRECISIONS[precision]
     return cfg
+
+
+class DeviceContextGraph:
+    """A context biasing graph uploaded to the device once (include/rvb_b200.h rvb_context_graph_*), for searches
+    whose vocabulary has `vocab` entries and whose blank is `blank_id`.  Built from either graph form
+    (context_graph.device_tables); a malformed graph raises ValueError before anything reaches the device.  The native
+    handle is freed with this object, after the searches enqueued with it have finished."""
+
+    def __init__(self, graph, vocab: int, blank_id: int = 0, device: Optional[torch.device] = None):
+        from .context_graph import check_device_tables, device_tables
+        t = device_tables(graph)
+        check_device_tables(t, int(vocab), int(blank_id))
+        self.lib = _lib.load()
+        self.vocab, self.blank_id, self.num_states = int(vocab), int(blank_id), int(t["fail"].shape[0])
+        self._h = None
+        a = {k: np.ascontiguousarray(v, dtype=np.float64 if v.dtype == np.float64 else np.int32) for k, v in t.items()}
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            h = self.lib.rvb_context_graph_create(self.num_states, _np_ptr(a["off"]), _np_ptr(a["tok"]),
+                                                  _np_ptr(a["dst"]), _np_ptr(a["fail"]), _np_ptr(a["bonus"]),
+                                                  _np_ptr(a["emit"]), _np_ptr(a["token_score"]), self.vocab,
+                                                  self.blank_id)
+        if not h:
+            raise ValueError("rvb_context_graph_create failed: " + _lib.last_error())
+        self._h = C.c_void_p(h)
+
+    def __del__(self):
+        try:
+            if self._h is not None:
+                self.lib.rvb_context_graph_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+# host graph -> {(device index, vocab, blank): DeviceContextGraph}: a graph object is uploaded once, not per batch
+_device_graphs: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
 
 
 class Engine:
@@ -273,10 +310,27 @@ class Engine:
                   "rvb_ctc_greedy_search")
         return [toks[b, :olen[b]].tolist() for b in range(B)]
 
+    def device_context_graph(self, graph, blank_id: int = 0) -> DeviceContextGraph:
+        """The device copy of a context graph (either form, or a DeviceContextGraph, returned as it is), uploaded on
+        first use and cached for as long as the host graph object lives."""
+        if isinstance(graph, DeviceContextGraph):
+            if graph.blank_id != int(blank_id):
+                raise ValueError(f"context graph was checked against blank {graph.blank_id}, the search uses {blank_id}")
+            return graph
+        key = (self.device.index, self.vocab, int(blank_id))
+        try:
+            per_graph = _device_graphs.setdefault(graph, {})
+        except TypeError:                                  # not weak-referenceable: upload for this call only
+            return DeviceContextGraph(graph, self.vocab, blank_id, self.device)
+        dg = per_graph.get(key)
+        if dg is None:
+            dg = per_graph[key] = DeviceContextGraph(graph, self.vocab, blank_id, self.device)
+        return dg
+
     def prefix_beam_search_raw(self, topk_val: torch.Tensor, topk_idx: torch.Tensor, enc_lens, beam: int,
-                               blank_id: int = 0):
+                               blank_id: int = 0, context=None):
         """n-best as arrays: tokens/times (B, beam, max_len) int32, lens (B, beam, 2) = {n_tokens, n_times},
-        scores (B, beam) float64, n_hyp (B,)."""
+        scores (B, beam) float64, n_hyp (B,).  context: a context graph (biased search, see device_context_graph)."""
         B, Tp, k = topk_idx.shape
         lens = np.ascontiguousarray(np.asarray(enc_lens, dtype=np.int32))
         max_len = max(int(lens.max()) if B else 1, 1)
@@ -285,17 +339,26 @@ class Engine:
         olen = np.zeros((B, beam, 2), dtype=np.int32)
         scores = np.zeros((B, beam), dtype=np.float64)
         nhyp = np.zeros(B, dtype=np.int32)
+        dg = None if context is None else self.device_context_graph(context, blank_id)
         with torch.cuda.device(self.device):
-            check(self.lib.rvb_ctc_prefix_beam_search(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp, beam,
-                                                      int(blank_id), max_len, _np_ptr(toks), _np_ptr(tims),
-                                                      _np_ptr(olen), _np_ptr(scores), _np_ptr(nhyp), self._stream()),
-                  "rvb_ctc_prefix_beam_search")
+            if dg is None:
+                check(self.lib.rvb_ctc_prefix_beam_search(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp, beam,
+                                                          int(blank_id), max_len, _np_ptr(toks), _np_ptr(tims),
+                                                          _np_ptr(olen), _np_ptr(scores), _np_ptr(nhyp), self._stream()),
+                      "rvb_ctc_prefix_beam_search")
+            else:
+                check(self.lib.rvb_ctc_prefix_beam_search_biased(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp,
+                                                                 beam, int(blank_id), max_len, _np_ptr(toks),
+                                                                 _np_ptr(tims), _np_ptr(olen), _np_ptr(scores),
+                                                                 _np_ptr(nhyp), dg._h, self._stream()),
+                      "rvb_ctc_prefix_beam_search_biased")
         return toks, tims, olen, scores, nhyp
 
     def prefix_beam_search(self, topk_val: torch.Tensor, topk_idx: torch.Tensor, enc_lens, beam: int,
-                           blank_id: int = 0):
+                           blank_id: int = 0, context=None):
         """-> per utterance (nbest tokens [tuple], nbest scores [float], nbest times [list])."""
-        toks, tims, olen, scores, nhyp = self.prefix_beam_search_raw(topk_val, topk_idx, enc_lens, beam, blank_id)
+        toks, tims, olen, scores, nhyp = self.prefix_beam_search_raw(topk_val, topk_idx, enc_lens, beam, blank_id,
+                                                                     context)
         out = []
         for b in range(toks.shape[0]):
             n = int(nhyp[b])
@@ -307,18 +370,24 @@ class Engine:
     # ---- prefix beam search (+ attention rescoring) as three stages around a native ticket, so that one host thread
     # can software-pipeline consecutive batches (asr_model.ASRModel.decode_stream): see include/rvb_b200.h
     def search_submit(self, topk_val: torch.Tensor, topk_idx: torch.Tensor, enc_out: torch.Tensor, enc_lens, beam: int,
-                      blank_id: int = 0) -> dict:
-        """Enqueue ctc_prefix_beam_search; returns the ticket (a dict that keeps every buffer of the batch alive)."""
+                      blank_id: int = 0, context=None) -> dict:
+        """Enqueue ctc_prefix_beam_search (biased by the context graph `context` when given); returns the ticket (a
+        dict that keeps every buffer of the batch, and the device graph, alive)."""
         B, Tp, k = topk_idx.shape
         lens = np.ascontiguousarray(np.asarray(enc_lens, dtype=np.int32))
         enc_out = enc_out.contiguous()
+        dg = None if context is None else self.device_context_graph(context, blank_id)
         with torch.cuda.device(self.device):
-            tid = self.lib.rvb_search_submit(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out), _np_ptr(lens), B, Tp,
-                                             beam, int(blank_id), self._stream())
+            if dg is None:
+                tid = self.lib.rvb_search_submit(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out), _np_ptr(lens),
+                                                 B, Tp, beam, int(blank_id), self._stream())
+            else:
+                tid = self.lib.rvb_search_submit_biased(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out),
+                                                        _np_ptr(lens), B, Tp, beam, int(blank_id), dg._h, self._stream())
         if tid < 0:
             raise RuntimeError("rvb_search_submit failed: " + _lib.last_error())
         return {"id": tid, "B": B, "Tp": Tp, "beam": beam, "cap": max(int(lens.max()) if B else 1, 1),
-                "keep": (topk_val, topk_idx, enc_out, lens), "stage": 1}
+                "keep": (topk_val, topk_idx, enc_out, lens, dg), "stage": 1}
 
     def rescoring_submit(self, t: dict, cat_embs=None, reverse_weight: float = 0.0, run_decoder: bool = True) -> None:
         """Wait for the hypothesis lengths of ticket `t`, then enqueue the decoder passes (attention rescoring) and the

@@ -48,6 +48,11 @@ def get_args(argv=None):
                    help="0.0 = nonverbatim ... 1.0 = verbatim; passed to the language-specific layers")
     p.add_argument("--timings_adjustment", type=float, default=230,
                    help="Subtract timings_adjustment milliseconds from each timestamp")
+    p.add_argument("--context_list_path", default=None,
+                   help="Phrases to boost (names, product terms, jargon), one per line; applies to "
+                        "ctc_prefix_beam_search and attention_rescoring")
+    p.add_argument("--context_graph_score", type=float, default=6.0,
+                   help="Bonus per matched token of a --context_list_path phrase")
     p.add_argument("--log_level", choices=["DEBUG", "INFO", "WARNING", "ERROR", "CRITICAL"], default="INFO")
     return p.parse_args(argv)
 
@@ -71,13 +76,14 @@ def main(argv=None):
         out_dir = os.path.join(args.result_dir, mode)
         os.makedirs(out_dir, exist_ok=True)
         targets[mode] = Path(out_dir) / Path(args.audio_file).with_suffix(".ctm").name
+    graph = asr.context_graph(args.context_list_path, args.context_graph_score) if args.context_list_path else None
     outputs = asr.transcribe_modes(
         args.audio_file, modes=args.modes, format="ctm", verbatimicity=args.verbatimicity,
         chunk_size=args.chunk_size, batch_size=args.batch_size, beam_size=args.beam_size,
         decoding_chunk_size=args.decoding_chunk_size, num_decoding_left_chunks=args.num_decoding_left_chunks,
         ctc_weight=args.ctc_weight, simulate_streaming=args.simulate_streaming, reverse_weight=args.reverse_weight,
         blank_penalty=args.blank_penalty, length_penalty=args.length_penalty,
-        timings_adjustment=args.timings_adjustment)
+        timings_adjustment=args.timings_adjustment, context_graph=graph)
     for mode, text in zip(args.modes, outputs):
         with targets[mode].open(mode="w") as fp:
             fp.write(text)

@@ -27,6 +27,7 @@ import torch.nn.functional as F
 import yaml
 
 from .asr_model import ASRModel, alignment_result
+from .context_graph import ContextGraph, tokenize
 from .ctc_align import adjust_model_time_offset, ctc_align, ctc_align_ms, frames_to_ms, hyps_to_ctm, hyps_to_txt
 from .engine import Engine, check_alignable, check_beam_size
 from .search import DecodeResult
@@ -163,8 +164,12 @@ class ReverbASR:
                          chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
                          decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                          simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
-                         length_penalty: float = 0.0, timings_adjustment: float = 230) -> list[str]:
+                         length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None) -> list[str]:
+        """context_graph: phrases to boost in ctc_prefix_beam_search / attention_rescoring (ReverbASR.context_graph, or
+        either ContextGraph form); the other modes ignore it, like the reference's decode()."""
         check_beam_size(beam_size)        # fail before any audio is read / decoded (limit: engine.MAX_BEAM_SIZE)
+        if context_graph is not None:     # upload (and check) the graph once, before any audio is decoded
+            context_graph = self.engine.device_context_graph(context_graph, self.blank_id)
         fc = self.test_conf["fbank_conf"]
         feats = self.compute_feats(audio_file, num_mel_bins=fc["num_mel_bins"], frame_length=fc["frame_length"],
                                    frame_shift=fc["frame_shift"])
@@ -173,7 +178,7 @@ class ReverbASR:
 
             kw = dict(decoding_chunk_size=decoding_chunk_size, num_decoding_left_chunks=num_decoding_left_chunks,
                       ctc_weight=ctc_weight, simulate_streaming=simulate_streaming, reverse_weight=reverse_weight,
-                      context_graph=None, blank_id=self.blank_id, blank_penalty=blank_penalty,
+                      context_graph=context_graph, blank_id=self.blank_id, blank_penalty=blank_penalty,
                       length_penalty=length_penalty, infos={"tasks": ["transcribe"], "langs": ["en"]}, cat_embs=cat_embs)
 
             def decode_batch(model, batch):
@@ -194,13 +199,20 @@ class ReverbASR:
                    verbatimicity: float = 1.0, chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
                    decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                    simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
-                   length_penalty: float = 0.0, timings_adjustment: float = 230) -> str:
+                   length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None) -> str:
         return self.transcribe_modes(
             audio_file, modes=[mode], format=format, verbatimicity=verbatimicity, chunk_size=chunk_size,
             batch_size=batch_size, beam_size=beam_size, decoding_chunk_size=decoding_chunk_size,
             num_decoding_left_chunks=num_decoding_left_chunks, ctc_weight=ctc_weight,
             simulate_streaming=simulate_streaming, reverse_weight=reverse_weight, blank_penalty=blank_penalty,
-            length_penalty=length_penalty, timings_adjustment=timings_adjustment)[0]
+            length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph)[0]
+
+    def context_graph(self, phrases, score: float = 6.0) -> ContextGraph:
+        """A context biasing graph over `phrases` — a file with one phrase per line, or a list of strings — tokenized
+        with this model's symbol table and sentencepiece model like the reference's ContextGraph; `score` is the bonus
+        per matched token.  Pass it as `context_graph=` to transcribe / transcribe_modes."""
+        bpe = self.configs["tokenizer_conf"].get("bpe_path")
+        return ContextGraph(context_score=score, token_lists=tokenize(phrases, self.tokenizer.symbol_table, bpe))
 
 
     def transcript_ids(self, transcript) -> List[int]:

@@ -84,10 +84,9 @@ class _Prefix:
 def ctc_prefix_beam_search_biased(topk_val: np.ndarray, topk_idx: np.ndarray, lens: Sequence[int], beam_size: int,
                                   context_graph, blank_id: int = 0) -> List[DecodeResult]:
     """CTC prefix beam search WITH a context graph (search.py:124-248, the `context_graph is not None` branches), on the
-    host over the per-frame top-`beam_size` log-probabilities the GPU CTC head produced — the biasing state machine is a
-    pointer-chasing automaton per prefix, and the reference itself only reaches this path through
-    `ASRModel.decode(context_graph=...)`, never from the reverb CLI.  topk_val / topk_idx: (B, T', beam) in `torch.topk`
-    order.  Reference behaviours kept: ranking by score + context score; the `u == last` repeat branch never updates
+    host over the per-frame top-`beam_size` log-probabilities the GPU CTC head produced.  `ASRModel.decode` runs the
+    biased GPU search (csrc/ctc.cu, csrc/context.cu) instead; this restatement is what the tests compare it against.
+    topk_val / topk_idx: (B, T', beam) in `torch.topk` order.  Reference behaviours kept: ranking by score + context score; the `u == last` repeat branch never updates
     `v_ns` (the `vs_ns` typo, :177); after the last frame `finalize` REPLACES each hypothesis' context score by minus the
     bonus of its unfinished match (:228-233) and the list is not re-sorted."""
     out: List[DecodeResult] = []

@@ -278,3 +278,47 @@ def write_wav(path: str, pcm: np.ndarray, sample_rate: int = 16000) -> str:
         w.setframerate(sample_rate)
         w.writeframes(np.ascontiguousarray(pcm, dtype=np.int16).tobytes())
     return path
+
+
+def context_phrases(n: int, vocab: int, seed: int = 0, blank_id: int = 0, max_len: int = 4):
+    """`n` seeded biasing phrases of 1..max_len non-blank token ids (duplicates and shared prefixes included, as in a
+    real list) — for the context biasing tests and tools/context_bench.py."""
+    rng = np.random.default_rng(seed)
+    toks = np.setdiff1d(np.arange(vocab), [blank_id])
+    return [rng.choice(toks, size=int(rng.integers(1, max_len + 1))).tolist() for _ in range(n)]
+
+
+def context_topk(B: int, T: int, k: int, vocab: int, phrases, seed: int = 0, blank_id: int = 0):
+    """Seeded per-frame top-k CTC log-probs (val (B, T, k) float32 descending, idx (B, T, k) int32) in which the tokens
+    of `phrases` appear often: every utterance walks through a script of phrase tokens and random tokens, each held a
+    few frames between blank runs; the script token is ranked first or, about a third of the time, just below a
+    competitor by a small margin — where a context bonus can change the n-best."""
+    rng = np.random.default_rng(seed)
+    pool = np.unique(np.concatenate([np.asarray(p, dtype=np.int64) for p in phrases] + [np.arange(vocab)]))
+    pool = pool[pool != blank_id]
+    idx = np.empty((B, T, k), dtype=np.int32)
+    val = np.empty((B, T, k), dtype=np.float32)
+    for b in range(B):
+        script = []
+        while len(script) < T:
+            script += list(phrases[int(rng.integers(len(phrases)))]) if rng.random() < 0.6 else \
+                rng.choice(pool, size=int(rng.integers(1, 4))).tolist()
+        pos, t = 0, 0
+        while t < T:
+            run = [blank_id] * int(rng.integers(0, 3)) + [script[pos]] * int(rng.integers(1, 4))
+            pos += 1
+            for tok in run[:T - t]:
+                others = rng.choice(pool, size=k + 1, replace=False)
+                others = [int(o) for o in others if o != tok][:k - 1]
+                if tok != blank_id and blank_id not in others and rng.random() < 0.7:
+                    others[-1] = blank_id
+                order = [tok] + others
+                if tok != blank_id and rng.random() < 0.35:
+                    order[0], order[1] = order[1], order[0]           # the script token trails a competitor
+                logits = np.sort(rng.normal(0.0, 1.0, k))[::-1] * 2.0
+                logits[0] = logits[1] + (rng.uniform(0.05, 1.0) if rng.random() < 0.5 else rng.uniform(1.0, 6.0))
+                lse = np.log(np.exp(logits - logits[0]).sum() + 1e-3) + logits[0]
+                idx[b, t] = order
+                val[b, t] = (logits - lse).astype(np.float32)
+                t += 1
+    return val, idx
