@@ -316,6 +316,16 @@ RVB_API int rvb_attention_tc(const void* d_q, const void* d_k, const void* d_v, 
 RVB_API int rvb_attention_tc_chunked(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk,
                                      int ldv, int ldo, int groups, int Tq, int Tk, int H, int dk, const float* d_key_bias,
                                      const int* d_k_lens, int chunk, int left_chunks, float scale, void* stream);
+/* For tests and tools: rvb_attention_tc with per-(query row, key) visibility bits on top of the key-length and causal
+ * masks, as the prefix-tree rescoring applies internally.  Bit (j & 31) of d_key_bits[(g*Tq + i) * bits_ld + (j >> 5)]
+ * (uint32, device) set <=> key j visible to query row i of group g; bits_ld >= 2 * ceil(Tk / 64). */
+RVB_API int rvb_attention_tc_bits(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk,
+                                  int ldv, int ldo, int groups, int Tq, int Tk, int H, int dk, const float* d_key_bias,
+                                  const int* d_k_lens, int causal, const void* d_key_bits, int bits_ld, float scale,
+                                  void* stream);
+/* For tests and tools: CTAs per SM of the wgmma attention instantiation a launch with these masks and Tk runs
+ * (chunk > 0: rvb_attention_tc_chunked; with_key_bits != 0: rvb_attention_tc_bits); -1 on error */
+RVB_API int rvb_attention_tc_blocks_per_sm(int Tk, int causal, int chunk, int with_key_bits);
 /* K'' = k + pos (bf16) and cbias[b,h,t] = u_h.k + v_h.pos for the folded rel-pos attention */
 RVB_API int rvb_relpos_prep(const void* d_k, int ldk, const void* d_pos, int ldp, const float* d_bias_u,
                             const float* d_bias_v, void* d_kpp, float* d_cbias, int B, int T, int H, int dk,

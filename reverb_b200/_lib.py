@@ -98,6 +98,9 @@ SIGNATURES = {
                            _i, _f, _vp]),
     "rvb_attention_tc_chunked": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _f, _vp]),
     "rvb_attention_tc": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _f, _vp]),
+    "rvb_attention_tc_bits": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i, _f,
+                                   _vp]),
+    "rvb_attention_tc_blocks_per_sm": (_i, [_i, _i, _i, _i]),
     "rvb_relpos_prep": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "rvb_f32_to_bf16": (_i, [_vp, _vp, _ll, _vp]),
     # include/rvb_diar.h

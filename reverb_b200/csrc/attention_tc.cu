@@ -7,18 +7,21 @@
 // so a small pre-kernel (or the projection GEMM's epilogue) builds K'' = k + p (bf16) and the per-key bias c (fp32)
 // once per layer, and the attention itself is ONE tensor-core product per key tile plus a key bias.
 //
-// Kernel (one CTA = 128 query rows of one (group, head), 288 threads):
-//   warp 8 / lane 0 : TMA producer — Q once, then K'' and V tiles of 64 keys through AT_ST-deep rings
-//   warps 0..7      : two consumer warpgroups of 64 query rows each; per key tile
-//                       S[64 x 64]  = Q . K''^T        wgmma m64n64k16 x 4, both operands from shared memory
-//                       online softmax on the S fragments in registers (scale, key bias, masks, running max / sum)
-//                       O[64 x 64] += P~ . V           wgmma m64n64k16 x 4, P~ (bf16) from registers, V MN-major
+// Kernel (one CTA = 128 query rows of one (group, head), 256 threads, two CTAs per SM):
+//   thread 0   : also issues the TMA loads — Q once, then K'' and V tiles of 64 keys through AT_ST-deep rings
+//   warps 0..7 : two warpgroups of 64 query rows each; per key tile
+//                  S[64 x 64]  = Q . K''^T        wgmma m64n64k16 x 4, both operands from shared memory
+//                  online softmax on the S fragments in registers (scale, key bias, masks, running max / sum)
+//                  O[64 x 64] += P~ . V           wgmma m64n64k16 x 4, P~ (bf16) from registers, V MN-major
+//                PV of tile j and S of tile j+1 go out as one wgmma group, so a warpgroup waits on the tensor cores
+//                once per tile; the other three warpgroups of the SM fill that wait.
 // Scores / probabilities never touch shared memory or HBM.
 #include <cuda.h>
 #include <math.h>
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "kernels.h"
 
@@ -28,7 +31,9 @@ constexpr int AT_BM = 128;  // query rows per CTA
 constexpr int AT_BN = 64;   // keys per tile
 constexpr int AT_DK = 64;
 constexpr int AT_ST = 4;    // K'' / V ring stages
-constexpr int AT_THREADS = 288;
+// Two warpgroups and no separate producer warp: the register file of each of the SM's four sub-partitions holds 16K
+// registers, so two CTAs of 8 warps (4 per sub-partition) may use 128 registers per thread, two CTAs of 9 warps only 96.
+constexpr int AT_THREADS = 256;
 constexpr uint32_t AT_Q_BYTES = AT_BM * AT_DK * 2;     // 16 KB
 constexpr uint32_t AT_TILE_BYTES = AT_BN * AT_DK * 2;  // 8 KB
 constexpr uint32_t AT_SMEM_FIXED = AT_Q_BYTES + 2 * AT_ST * AT_TILE_BYTES + 256 /*barriers*/ + 1024 /*align slack*/;
@@ -53,7 +58,23 @@ struct AttnTcParams {
   float scale_log2;
 };
 
-__global__ void __launch_bounds__(AT_THREADS, 1)
+// Which masks a launch applies on top of the key lengths.  Each kind is its own instantiation, so the encoder's
+// kernel carries no mask code.
+enum AttnMask : int {
+  MASK_LENS = 0,   // key lengths only (encoder self-attention, cross-attention)
+  MASK_CHUNK = 1,  // chunk / causal mask, p.chunk > 0
+  MASK_BITS = 2,   // key_bits, and the chunk / causal mask when p.chunk > 0 (prefix-tree self-attention)
+};
+
+// one S = Q . K''^T tile product into s (not committed)
+__device__ __forceinline__ void attn_issue_s(float* s, uint64_t qdesc, const uint8_t* k_tile) {
+  const uint64_t kdesc = make_sw128_desc(smem_u32(k_tile));
+#pragma unroll
+  for (int k = 0; k < AT_DK / 16; ++k) wgmma_m64n64k16_ss(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
+}
+
+template <int MASK>
+__global__ void __launch_bounds__(AT_THREADS, 2)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -76,21 +97,38 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   int klen = p.Tk;
   if (p.k_lens) klen = min(klen, __ldg(p.k_lens + g));
   // chunk mask: only the key tiles some row of this query tile can see are visited: [jt0, jt0 + ntiles)
-  auto vis_lo = [&](int i) { return (p.chunk > 0 && p.left >= 0) ? max(0, (i / p.chunk - p.left) * p.chunk) : 0; };
-  auto vis_hi = [&](int i) { return p.chunk > 0 ? min(klen, (i / p.chunk + 1) * p.chunk) : klen; };
+  const bool chunked = MASK == MASK_CHUNK || (MASK == MASK_BITS && p.chunk > 0);
+  auto vis_lo = [&](int i) { return (chunked && p.left >= 0) ? max(0, (i / p.chunk - p.left) * p.chunk) : 0; };
+  auto vis_hi = [&](int i) { return chunked ? min(klen, (i / p.chunk + 1) * p.chunk) : klen; };
   const int jt0 = vis_lo(q0) / AT_BN;
   const int ntiles = max(0, (vis_hi(q0 + AT_BM - 1) + AT_BN - 1) / AT_BN - jt0);
   const long long krow0 = (long long)g * p.Tk;
+  // K'' and V tile n into ring stage n % AT_ST (thread 0 only)
+  auto load_tile = [&](int n) {
+    const int st = n % AT_ST;
+    const int krow = (int)(krow0 + (jt0 + n) * AT_BN);
+    mbar_expect_tx(&k_full[st], AT_TILE_BYTES);
+    tma_load_2d(sK + st * AT_TILE_BYTES, &tmK, &k_full[st], h * AT_DK, krow);
+    mbar_expect_tx(&v_full[st], AT_TILE_BYTES);
+    tma_load_2d(sV + st * AT_TILE_BYTES, &tmV, &v_full[st], h * AT_DK, krow);
+  };
 
+  // Thread 0 issues every load: Q and the first AT_ST tiles right after the barrier init, so they are in flight while
+  // the key-bias table is filled; later tiles from the main loop.
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int i = 0; i < AT_ST; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 8);   // lane 0 of every consumer warp
+      mbar_init(&k_empty[i], 8);   // lane 0 of every warp
       mbar_init(&v_full[i], 1);
       mbar_init(&v_empty[i], 8);
     }
     fence_barrier_init();
+    if (ntiles > 0) {
+      mbar_expect_tx(q_full, AT_Q_BYTES);
+      tma_load_2d(sQ, &tmQ, q_full, h * AT_DK, (int)((long long)g * p.Tq + q0));
+      for (int n = 0; n < min(ntiles, AT_ST); ++n) load_tile(n);
+    }
   }
   {
     // key bias row of this (group, head), pre-scaled; masked keys -> -inf
@@ -102,29 +140,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == 8) {
-    // ---------------------------------------------------------------- TMA producer
-    if (lane == 0 && ntiles > 0) {
-      tma_prefetch_desc(&tmQ);
-      tma_prefetch_desc(&tmK);
-      tma_prefetch_desc(&tmV);
-      mbar_expect_tx(q_full, AT_Q_BYTES);
-      tma_load_2d(sQ, &tmQ, q_full, h * AT_DK, (int)((long long)g * p.Tq + q0));
-      for (int n = 0; n < ntiles; ++n) {
-        const int st = n % AT_ST, ph = ((n / AT_ST) & 1) ^ 1;
-        const int krow = (int)(krow0 + (jt0 + n) * AT_BN);
-        mbar_wait(&k_empty[st], ph);
-        mbar_expect_tx(&k_full[st], AT_TILE_BYTES);
-        tma_load_2d(sK + st * AT_TILE_BYTES, &tmK, &k_full[st], h * AT_DK, krow);
-        mbar_wait(&v_empty[st], ph);
-        mbar_expect_tx(&v_full[st], AT_TILE_BYTES);
-        tma_load_2d(sV + st * AT_TILE_BYTES, &tmV, &v_full[st], h * AT_DK, krow);
-      }
-    }
-    return;
-  }
-
-  // ------------------------------------------------------------------ consumer warpgroups
   const int wg = warp >> 2, wl = warp & 3;
   // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16) and its key / dk columns
   // 8j + 2(l%4) + {0, 1}, j = 0..7
@@ -135,25 +150,33 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, row_sum[2] = {0.f, 0.f};   // row_sum: this thread's columns only
-  if (ntiles > 0) mbar_wait(q_full, 0);
   const uint64_t qdesc = make_sw128_desc(smem_u32(sQ + wg * (AT_Q_BYTES / 2)));
-#pragma unroll 1
-  for (int j = 0; j < ntiles; ++j) {
+  // s holds S of the tile being worked on; S(0) goes out here, S(j+1) with PV(j)
+  float s[32];
+  if (ntiles > 0) {
+    mbar_wait(q_full, 0);
+    mbar_wait(&k_full[0], 0);
+    wgmma_fence_regs<32>(s);
+    wgmma_fence();
+    attn_issue_s(s, qdesc, sK);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs<32>(s);
+    if (lane == 0) mbar_arrive(&k_empty[0]);
+  }
+  // one key tile; NEXT (every tile but the last) also issues S(j+1).  The last tile is a separate copy, so no branch
+  // sits between the products of one wgmma group.
+  auto tile = [&](const int j, auto next_tag) {
+    constexpr bool next = decltype(next_tag)::value;
     const int st = j % AT_ST, ph = (j / AT_ST) & 1;
-    // ---- S = Q . K''^T
-    float s[32];
-    mbar_wait(&k_full[st], ph);
-    {
-      const uint64_t kdesc = make_sw128_desc(smem_u32(sK + st * AT_TILE_BYTES));
-      wgmma_fence_regs<32>(s);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < AT_DK / 16; ++k) wgmma_m64n64k16_ss(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs<32>(s);
+    // ---- refill the stage of tile j - 1 once all 8 warps have released it; the ring stays AT_ST - 1 tiles ahead
+    if (threadIdx.x == 0 && j > 0 && j - 1 + AT_ST < ntiles) {
+      const int n = j - 1 + AT_ST, ph_free = ((n / AT_ST) & 1) ^ 1;
+      mbar_wait(&k_empty[n % AT_ST], ph_free);
+      mbar_wait(&v_empty[n % AT_ST], ph_free);
+      load_tile(n);
     }
-    if (lane == 0) mbar_arrive(&k_empty[st]);
+    __syncwarp();
     // ---- x = s * scale*log2e + key bias, masks, tile maximum per row
     const int kbase = (jt0 + j) * AT_BN;
     const float* bias = s_bias + j * AT_BN;
@@ -167,7 +190,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         s[4 * jj + 2 * i + 1] = fmaf(s[4 * jj + 2 * i + 1], p.scale_log2, b2.y);
       }
     }
-    if (p.chunk > 0) {
+    if (chunked) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int lo = vis_lo(row[i]) - kbase, hi = vis_hi(row[i]) - kbase;   // visible columns: lo <= c < hi
@@ -180,7 +203,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           }
       }
     }
-    if (p.key_bits) {
+    if (MASK == MASK_BITS) {
       // arbitrary visibility (prefix-tree self-attention: a node sees its ancestors): one bit per key of the row
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -234,21 +257,33 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         row_sum[i] += pr.x + pr.y;
         pa[2 * jj + i] = w;   // ks = jj / 2: regs {jj even: a0 (row), a1 (row + 8); jj odd: a2, a3}
       }
-    // ---- O += P~ . V
+    // ---- O += P~ . V, then S of the next tile into s (free now that P~ is packed); groups retire in order, so one
+    // wait covers both
+    const int st1 = (j + 1) % AT_ST;
     mbar_wait(&v_full[st], ph);
+    if (next) mbar_wait(&k_full[st1], ((j + 1) / AT_ST) & 1);
     {
       const uint64_t vdesc = make_sw128_desc(smem_u32(sV + st * AT_TILE_BYTES));
       wgmma_fence_regs<32>(o);
+      wgmma_fence_regs<32>(s);
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < AT_BN / 16; ++ks)
         wgmma_m64n64k16_rs_tb(o, pa + 4 * ks, vdesc + (uint64_t)((ks * 16 * 128) >> 4));   // 16 key rows of 128 B
+      if (next) attn_issue_s(s, qdesc, sK + st1 * AT_TILE_BYTES);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs<32>(o);
+      wgmma_fence_regs<32>(s);
     }
-    if (lane == 0) mbar_arrive(&v_empty[st]);
-  }
+    if (lane == 0) {
+      mbar_arrive(&v_empty[st]);
+      if (next) mbar_arrive(&k_empty[st1]);
+    }
+  };
+#pragma unroll 1
+  for (int j = 0; j + 1 < ntiles; ++j) tile(j, std::true_type());
+  if (ntiles > 0) tile(ntiles - 1, std::false_type());
   // ---- epilogue: O / row_sum -> bf16 -> global (rows without a visible key: zeros)
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -375,6 +410,44 @@ static int tmap_2d(CUtensorMap* m, const void* base, long long cols, long long r
   return 0;
 }
 
+static int attn_mask_kind(bool chunk_or_causal, bool key_bits) {
+  return key_bits ? MASK_BITS : chunk_or_causal ? MASK_CHUNK : MASK_LENS;
+}
+
+// Q, both rings, barriers and the key-bias row: 86 272 B at Tk = 748.  Two CTAs fit the 228 KB of an SM (1 KB of it
+// reserved per CTA) up to Tk = 8 128; longer key rows run one CTA per SM.
+static size_t attn_smem_bytes(int Tk) { return AT_SMEM_FIXED + (size_t)((Tk + AT_BN - 1) / AT_BN) * AT_BN * sizeof(float); }
+
+template <int MASK>
+static int attn_opt_in(size_t smem) {
+  static DynSmemOptIn optin;
+  return optin.ensure(attention_tc_kernel<MASK>, smem);
+}
+
+template <int MASK>
+static int attn_launch(dim3 grid, size_t smem, cudaStream_t stream, const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                       const CUtensorMap& tmV, const AttnTcParams& p) {
+  if (attn_opt_in<MASK>(smem)) return -1;
+  attention_tc_kernel<MASK><<<grid, AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
+  return 0;
+}
+
+template <int MASK>
+static int attn_blocks_per_sm(size_t smem, int* blocks) {
+  if (attn_opt_in<MASK>(smem)) return -1;
+  RVB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks, attention_tc_kernel<MASK>, AT_THREADS, smem));
+  return 0;
+}
+
+int attention_tc_blocks_per_sm(int Tk, bool chunk_or_causal, bool key_bits, int* blocks) {
+  const size_t smem = attn_smem_bytes(Tk);
+  switch (attn_mask_kind(chunk_or_causal, key_bits)) {
+    case MASK_LENS: return attn_blocks_per_sm<MASK_LENS>(smem, blocks);
+    case MASK_CHUNK: return attn_blocks_per_sm<MASK_CHUNK>(smem, blocks);
+    default: return attn_blocks_per_sm<MASK_BITS>(smem, blocks);
+  }
+}
+
 // q: (groups*Tq, ldq) rows with head h at columns [h*64, h*64+64) (+ the pointer offset already applied), same for k, v.
 int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
   RVB_REQUIRE(a.dk == AT_DK, "attention_tc: only d_k = 64 is built");
@@ -411,11 +484,15 @@ int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
   if (tmap_2d(&tmK, a.k, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldk, AT_BN)) return -1;
   if (tmap_2d(&tmV, a.v, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldv, AT_BN)) return -1;
   dim3 grid((a.Tq + AT_BM - 1) / AT_BM, a.H, a.groups);
-  const size_t smem = AT_SMEM_FIXED + (size_t)((a.Tk + AT_BN - 1) / AT_BN) * AT_BN * sizeof(float);
+  const size_t smem = attn_smem_bytes(a.Tk);
   RVB_REQUIRE(smem <= 227 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
-  static DynSmemOptIn optin;
-  if (optin.ensure(attention_tc_kernel, smem)) return -1;
-  attention_tc_kernel<<<grid, AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
+  int rc;
+  switch (attn_mask_kind(a.causal || a.chunk > 0, a.key_bits != nullptr)) {
+    case MASK_LENS: rc = attn_launch<MASK_LENS>(grid, smem, stream, tmQ, tmK, tmV, p); break;
+    case MASK_CHUNK: rc = attn_launch<MASK_CHUNK>(grid, smem, stream, tmQ, tmK, tmV, p); break;
+    default: rc = attn_launch<MASK_BITS>(grid, smem, stream, tmQ, tmK, tmV, p); break;
+  }
+  if (rc) return rc;
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
   return 0;

@@ -2320,6 +2320,33 @@ RVB_API int rvb_attention_tc(const void* d_q, const void* d_k, const void* d_v, 
   return rvb::launch_attention_tc(a, (cudaStream_t)stream);
 }
 
+RVB_API int rvb_attention_tc_bits(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk,
+                                  int ldv, int ldo, int groups, int Tq, int Tk, int H, int dk, const float* d_key_bias,
+                                  const int* d_k_lens, int causal, const void* d_key_bits, int bits_ld, float scale,
+                                  void* stream) {
+  rvb::AttnTcArgs a;
+  a.q = reinterpret_cast<const rvb::bf16*>(d_q);
+  a.k = reinterpret_cast<const rvb::bf16*>(d_k);
+  a.v = reinterpret_cast<const rvb::bf16*>(d_v);
+  a.out = reinterpret_cast<rvb::bf16*>(d_out);
+  a.ldq = ldq; a.ldk = ldk; a.ldv = ldv; a.ldo = ldo;
+  a.groups = groups; a.Tq = Tq; a.Tk = Tk; a.H = H; a.dk = dk;
+  a.key_bias = d_key_bias;
+  a.k_lens = d_k_lens;
+  a.causal = causal;
+  a.key_bits = reinterpret_cast<const uint32_t*>(d_key_bits);
+  a.bits_ld = bits_ld;
+  a.scale = scale;
+  RVB_REQUIRE(d_key_bits != nullptr, "rvb_attention_tc_bits: d_key_bits is null");
+  return rvb::launch_attention_tc(a, (cudaStream_t)stream);
+}
+
+RVB_API int rvb_attention_tc_blocks_per_sm(int Tk, int causal, int chunk, int with_key_bits) {
+  int blocks = 0;
+  if (rvb::attention_tc_blocks_per_sm(Tk, causal || chunk > 0, with_key_bits != 0, &blocks)) return -1;
+  return blocks;
+}
+
 RVB_API int rvb_attention_tc_chunked(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk,
                                      int ldv, int ldo, int groups, int Tq, int Tk, int H, int dk, const float* d_key_bias,
                                      const int* d_k_lens, int chunk, int left_chunks, float scale, void* stream) {

@@ -192,6 +192,8 @@ struct AttnTcArgs {
   float scale = 1.0f;
 };
 int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream);
+// CTAs per SM of the instantiation launch_attention_tc runs for these masks and Tk
+int attention_tc_blocks_per_sm(int Tk, bool chunk_or_causal, bool key_bits, int* blocks);
 // K'' = k + pos (bf16, (B*T, H*dk) dense) and cbias[b,h,t] = u_h . k + v_h . pos
 int launch_relpos_prep(const bf16* k, int ldk, const bf16* pos, int ldp, const float* bias_u, const float* bias_v,
                        bf16* kpp, float* cbias, int B, int T, int H, int dk, cudaStream_t stream);
