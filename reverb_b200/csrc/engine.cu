@@ -174,7 +174,7 @@ struct rvb_model {
   int pall_T = 0;               // ws_pall holds linear_pos(pos_emb) for this many frames
   const void* pall_ptr = nullptr;
   int lens_slot = 0;
-  int lens_B = 0;
+  int lens_cap = 0;             // batch rows per slot of the pinned length ring (the largest B seen)
   static constexpr int kTickets = 4;
   rvb::SearchTicket* tickets = nullptr;  // [kTickets], created on first use (engine.cu search_submit)
   rvb::DecCache* dcache = nullptr;        // KV cache of the autoregressive decoder (decoder_cache_begin / _step)
@@ -545,21 +545,22 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
   if (fold_lang(m, h_cat, n_cat, stream)) return -1;
 
   // lengths
-  // pinned staging ring: a back-to-back call must not overwrite lengths an earlier async copy still reads
+  // pinned staging ring: a back-to-back call must not overwrite lengths an earlier async copy still reads.  Slots are
+  // sized for the largest batch seen, so batches of varying B (corpus decoding) only wait when that maximum grows.
   constexpr int kRing = 16;
-  if (m->pin_a.ensure(sizeof(int) * B * kRing) || m->ws_lens.ensure(sizeof(int) * B * kRing)) return -1;
-  if (m->lens_B != B) {
+  if (B > m->lens_cap) {
     RVB_CHECK_CUDA(cudaStreamSynchronize(stream));
-    m->lens_B = B;
+    if (m->pin_a.ensure(sizeof(int) * B * kRing) || m->ws_lens.ensure(sizeof(int) * B * kRing)) return -1;
+    m->lens_cap = B;
   }
   const int slot = (m->lens_slot++) % kRing;
-  int* h_lens = m->pin_a.as<int>() + (size_t)slot * B;
+  int* h_lens = m->pin_a.as<int>() + (size_t)slot * m->lens_cap;
   for (int b = 0; b < B; ++b) {
     int e = rvb_encoder_out_len(h_feat_lens[b], T);
     h_lens[b] = e;
     if (h_enc_lens) h_enc_lens[b] = e;
   }
-  int* d_lens = m->ws_lens.as<int>() + (size_t)slot * B;
+  int* d_lens = m->ws_lens.as<int>() + (size_t)slot * m->lens_cap;
   RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, h_lens, sizeof(int) * B, cudaMemcpyHostToDevice, stream));
 
   // workspace
@@ -610,8 +611,9 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     }
     m->pe_T = Tp;
   }
-  // ... which depends on the frame count only: kept across calls of the same shape
-  if (m->pall_T != Tp || m->pall_ptr != (const void*)pall) {
+  // ... where row t depends on t only (the GEMM computes rows independently): kept for the longest T' seen, and a
+  // shorter batch reads its leading rows
+  if (m->pall_T < Tp || m->pall_ptr != (const void*)pall) {
     if (gemm(m, m->ws_pe.as<bf16>(), m->pos_all, Tp, ACT_NONE, OUT_BF16, pall, 1.f, stream, nullptr, 0, 0, false))
       return -1;
     m->pall_T = Tp;

@@ -2,6 +2,7 @@
 asr/wenet/bin/recognize_wav.py (flags :33-145, `<result_dir>/<mode>/<audio stem>.ctm` :177-204).
 
     python -m reverb_b200.recognize_wav --model <dir> --audio_file a.wav --result_dir out
+    python -m reverb_b200.recognize_wav --model <dir> --audio_file calls/*.wav --result_dir out   # batched together
 """
 from __future__ import annotations
 
@@ -16,7 +17,8 @@ MODES = ["attention", "ctc_greedy_search", "ctc_prefix_beam_search", "attention_
 def get_args(argv=None):
     from .reverb import get_available_models
     p = argparse.ArgumentParser(description="Run automatic speech recognition on a given wav file using the Rev model.")
-    p.add_argument("--audio_file", required=True, help="Audio to transcribe")
+    p.add_argument("--audio_file", required=True, nargs="+",
+                   help="Audio to transcribe; several files are decoded together, in shared batches")
     p.add_argument("--config", default=None, help="Path to config file")
     p.add_argument("--checkpoint", default=None, help="Path to Reverb model checkpoint")
     p.add_argument("--model", default=None,
@@ -57,8 +59,20 @@ def get_args(argv=None):
     return p.parse_args(argv)
 
 
+def output_names(audio_files) -> list:
+    """`<stem>.ctm` of every input; two inputs with the same stem would write the same file."""
+    names = [Path(f).with_suffix(".ctm").name for f in audio_files]
+    seen = {}
+    for f, n in zip(audio_files, names):
+        if n in seen:
+            raise ValueError(f"--audio_file {seen[n]} and {f} would both write {n}")
+        seen[n] = f
+    return names
+
+
 def main(argv=None):
     args = get_args(argv)
+    names = output_names(args.audio_file)
     logging.basicConfig(level=args.log_level, format="%(asctime)s %(filename)s %(levelname)s: %(message)s")
     from .reverb import ReverbASR, load_model
     by_name = args.model is not None
@@ -71,22 +85,22 @@ def main(argv=None):
         asr = ReverbASR(args.config, args.checkpoint, cmvn_path=args.cmvn_path,
                         tokenizer_symbols=args.tokenizer_symbols, bpe_path=args.bpe_path, gpu=args.gpu,
                         overwrite_cmvn=args.overwrite_cmvn)
-    targets = {}
+    out_dirs = []
     for mode in args.modes:
-        out_dir = os.path.join(args.result_dir, mode)
-        os.makedirs(out_dir, exist_ok=True)
-        targets[mode] = Path(out_dir) / Path(args.audio_file).with_suffix(".ctm").name
+        out_dirs.append(Path(args.result_dir) / mode)
+        os.makedirs(out_dirs[-1], exist_ok=True)
     graph = asr.context_graph(args.context_list_path, args.context_graph_score) if args.context_list_path else None
-    outputs = asr.transcribe_modes(
+    results = asr.transcribe_files(
         args.audio_file, modes=args.modes, format="ctm", verbatimicity=args.verbatimicity,
         chunk_size=args.chunk_size, batch_size=args.batch_size, beam_size=args.beam_size,
         decoding_chunk_size=args.decoding_chunk_size, num_decoding_left_chunks=args.num_decoding_left_chunks,
         ctc_weight=args.ctc_weight, simulate_streaming=args.simulate_streaming, reverse_weight=args.reverse_weight,
         blank_penalty=args.blank_penalty, length_penalty=args.length_penalty,
         timings_adjustment=args.timings_adjustment, context_graph=graph)
-    for mode, text in zip(args.modes, outputs):
-        with targets[mode].open(mode="w") as fp:
-            fp.write(text)
+    for name, (_, outputs) in zip(names, results):
+        for out_dir, text in zip(out_dirs, outputs):
+            with (out_dir / name).open(mode="w") as fp:
+                fp.write(text)
 
 
 if __name__ == "__main__":

@@ -14,22 +14,27 @@ Differences that are deliberate and documented in DESIGN.md:
 from __future__ import annotations
 
 import logging
+import math
+import queue
 import shutil
+import threading
+from collections import deque
 from functools import partial
-from itertools import chain
 from math import ceil
 from pathlib import Path
-from typing import Dict, Generator, List, Tuple
+from typing import Dict, Generator, Iterator, List, Tuple
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 import yaml
 
+from . import corpus
 from .asr_model import ASRModel, alignment_result
 from .context_graph import ContextGraph, tokenize
 from .ctc_align import adjust_model_time_offset, ctc_align, ctc_align_ms, frames_to_ms, hyps_to_ctm, hyps_to_txt
 from .engine import Engine, check_alignable, check_beam_size
+from .resample import resampled_length
 from .search import DecodeResult
 from .text import get_blank_id, init_tokenizer
 
@@ -125,8 +130,13 @@ class ReverbASR:
     def compute_feats(self, audio_file: str, resample_rate: int = 16000, num_mel_bins=23, frame_length=25,
                       frame_shift=10, dither=0.0) -> torch.Tensor:
         """(1, m, num_mel_bins) float32 on the device; kernel: csrc/fbank.cu."""
-        if num_mel_bins != 80 or frame_length != 25 or frame_shift != 10 or dither != 0.0 or resample_rate != 16000:
-            raise NotImplementedError("reverb_b200 fbank kernel is built for 80 bins / 25 ms / 10 ms / no dither @16 kHz")
+        _check_fbank_conf(num_mel_bins, frame_length, frame_shift, dither, resample_rate)
+        rec = self._read_recording(audio_file, resample_rate)
+        return self._recording_feats(rec, resample_rate).unsqueeze(0)
+
+    def _read_recording(self, audio_file, resample_rate: int = 16000) -> "_Recording":
+        """Reads channel 0 of a recording on the host.  Raises the front end's error for a recording that has fewer
+        than 400 samples at `resample_rate`, before anything is uploaded."""
         pcm, sample_rate = _read_wav(audio_file)
         logging.info(f"detected sample rate: {sample_rate}")
         ch0 = np.array(pcm[0], copy=True)                      # channel 0 (kaldi.fbank channel=-1 -> 0)
@@ -134,13 +144,23 @@ class ReverbASR:
             # `waveform.to(torch.float)` of the reference (cli/reverb.py:124): the sample VALUES as they are (uint8 /
             # int32 / float32) — the kernels take int16 or float32 input
             ch0 = ch0.astype(np.float32)
-        wave_dev = torch.from_numpy(ch0).pin_memory().to(self.device, non_blocking=True)
+        n = ch0.shape[0]
         if sample_rate != resample_rate:
+            g = math.gcd(int(sample_rate), int(resample_rate))
+            n = resampled_length(n, int(sample_rate) // g, int(resample_rate) // g)
+        if n < 400:
+            raise AssertionError(f"choose a window size 400 that is [2, {n}]")  # torchaudio's check
+        return _Recording(audio_file, ch0, sample_rate, int(self.engine.lib.rvb_fbank_num_frames(n)))
+
+    def _recording_feats(self, rec: "_Recording", resample_rate: int = 16000) -> torch.Tensor:
+        """Upload, resampling and fbank of one recording on the current stream -> (m, 80) float32."""
+        wave_dev = torch.from_numpy(rec.pcm).pin_memory().to(self.device, non_blocking=True)
+        if rec.sample_rate != resample_rate:
             # torchaudio.transforms.Resample on channel 0 (the reference resamples every channel, then keeps the first)
-            wave_dev = self.engine.resample(wave_dev, sample_rate, resample_rate)
-        if wave_dev.numel() < 400:
-            raise AssertionError(f"choose a window size 400 that is [2, {wave_dev.numel()}]")  # torchaudio's check
-        return self.engine.fbank(wave_dev).unsqueeze(0)
+            wave_dev = self.engine.resample(wave_dev, rec.sample_rate, resample_rate)
+        feats = self.engine.fbank(wave_dev)
+        assert feats.shape[0] == rec.frames
+        return feats
 
     def feats_batcher(self, infeats: torch.Tensor, chunk_size: int, batch_size: int
                       ) -> Generator[Tuple[torch.Tensor, torch.Tensor], None, None]:
@@ -167,33 +187,123 @@ class ReverbASR:
                          length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None) -> list[str]:
         """context_graph: phrases to boost in ctc_prefix_beam_search / attention_rescoring (ReverbASR.context_graph, or
         either ContextGraph form); the other modes ignore it, like the reference's decode()."""
+        for _, outputs in self.transcribe_files(
+                [audio_file], modes, format=format, verbatimicity=verbatimicity, chunk_size=chunk_size,
+                batch_size=batch_size, beam_size=beam_size, decoding_chunk_size=decoding_chunk_size,
+                num_decoding_left_chunks=num_decoding_left_chunks, ctc_weight=ctc_weight,
+                simulate_streaming=simulate_streaming, reverse_weight=reverse_weight, blank_penalty=blank_penalty,
+                length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph):
+            pass
+        return outputs
+
+    def transcribe_files(self, audio_files, modes: List[str], format: str = "txt", verbatimicity: float = 1.0,
+                         chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
+                         decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
+                         simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
+                         length_penalty: float = 0.0, timings_adjustment: float = 230,
+                         context_graph=None) -> Iterator[Tuple[str, List[str]]]:
+        """Transcribes many recordings with one set of decode settings -> (audio_file, [output per mode]) in input
+        order, each as soon as it and every earlier recording are decoded.  Every output is the one
+        `transcribe_modes(audio_file, ...)` gives on its own.
+
+        Batches hold chunks of several recordings, and tail chunks run at a trimmed length (reverb_b200/corpus.py,
+        DESIGN.md §4f).  Files are read and parsed on a background thread, one window of recordings ahead; upload,
+        resampling, fbank and decoding run on the caller's thread and current stream (or the lanes of `set_lanes`).
+        A file that cannot be read, or has under 400 samples, raises the error `transcribe` raises, naming the file,
+        after the outputs of every earlier file; no batch holding its chunks is decoded."""
         check_beam_size(beam_size)        # fail before any audio is read / decoded (limit: engine.MAX_BEAM_SIZE)
-        if context_graph is not None:     # upload (and check) the graph once, before any audio is decoded
+        if context_graph is not None:     # upload (and check) the graph once, before any audio is read
             context_graph = self.engine.device_context_graph(context_graph, self.blank_id)
         fc = self.test_conf["fbank_conf"]
-        feats = self.compute_feats(audio_file, num_mel_bins=fc["num_mel_bins"], frame_length=fc["frame_length"],
-                                   frame_shift=fc["frame_shift"])
-        with torch.no_grad():
-            cat_embs = torch.tensor([verbatimicity, 1.0 - verbatimicity])
+        _check_fbank_conf(fc["num_mel_bins"], fc["frame_length"], fc["frame_shift"])
+        # tails keep the padded length where the padding is part of the result: simulate_streaming has no padding
+        # mask, and the attention mode's beam search runs up to T' steps
+        trim = not simulate_streaming and "attention" not in modes
+        right = corpus.right_context(self.configs["encoder_conf"])
+        cat_embs = torch.tensor([verbatimicity, 1.0 - verbatimicity])
+        kw = dict(decoding_chunk_size=decoding_chunk_size, num_decoding_left_chunks=num_decoding_left_chunks,
+                  ctc_weight=ctc_weight, simulate_streaming=simulate_streaming, reverse_weight=reverse_weight,
+                  context_graph=context_graph, blank_id=self.blank_id, blank_penalty=blank_penalty,
+                  length_penalty=length_penalty, infos={"tasks": ["transcribe"], "langs": ["en"]}, cat_embs=cat_embs)
 
-            kw = dict(decoding_chunk_size=decoding_chunk_size, num_decoding_left_chunks=num_decoding_left_chunks,
-                      ctc_weight=ctc_weight, simulate_streaming=simulate_streaming, reverse_weight=reverse_weight,
-                      context_graph=context_graph, blank_id=self.blank_id, blank_penalty=blank_penalty,
-                      length_penalty=length_penalty, infos={"tasks": ["transcribe"], "langs": ["en"]}, cat_embs=cat_embs)
+        def decode_batch(model, batch):
+            return model.decode(modes, batch[0], batch[1], beam_size, **kw)
 
-            def decode_batch(model, batch):
-                feats_batch, feats_lengths = batch
-                return model.decode(modes, feats_batch, feats_lengths, beam_size, **kw)
+        def window_batches(window):
+            return self._window_batches(window, chunk_size, batch_size, right, trim)
 
-            batches = self.feats_batcher(feats, chunk_size, batch_size)
+        reader = _Reader(self, list(audio_files), corpus.window_frames(batch_size, chunk_size))
+        waiting: deque = deque()             # recordings not yet yielded, in input order
+        stream = None
+        try:
+            # decode() and decode_stream run without autograd themselves; no grad-mode context spans a yield here
             if self._lanes is not None:
-                results = self._lanes.run(list(batches), decode_batch)
+                def decoded():
+                    for window in reader:
+                        waiting.extend(window)
+                        jobs = window_batches(window)
+                        for (plan, _, _), res in zip(jobs, self._lanes.run([job[1:] for job in jobs], decode_batch)):
+                            yield (plan, window), res
             else:
-                # the reference's sequential batch loop (cli/reverb.py:214-234), software-pipelined on one stream
-                results = list(self.model.decode_stream(batches, modes, beam_size, **kw))
-        return [get_output(format, self.tokenizer, Path(audio_file).name,
-                           list(chain(*(hyp[mode] for hyp in results))), timings_adjustment, chunk_size,
-                           self.input_frame_length, self.output_frame_length) for mode in modes]
+                plans: deque = deque()
+
+                def batches():
+                    for window in reader:
+                        waiting.extend(window)
+                        for plan, fb, fl in window_batches(window):
+                            plans.append((plan, window))
+                            yield fb, fl
+
+                # one software-pipelined decode_stream across window boundaries
+                stream = self.model.decode_stream(batches(), modes, beam_size, **kw)
+
+                def decoded():
+                    for res in stream:
+                        plan, window = plans.popleft()
+                        yield (plan, window), res
+
+            for (plan, window), res in decoded():
+                for s, (r, c) in enumerate(plan.slots):
+                    rec = window[r]
+                    for mode in modes:
+                        rec.hyps.setdefault(mode, {})[c] = res[mode][s]
+                    rec.left -= 1
+                while waiting and waiting[0].left == 0:
+                    rec = waiting.popleft()
+                    yield rec.path, [get_output(format, self.tokenizer, Path(rec.path).name,
+                                                [rec.hyps[mode][c] for c in range(rec.chunks)],
+                                                timings_adjustment, chunk_size, self.input_frame_length,
+                                                self.output_frame_length) for mode in modes]
+        finally:
+            if stream is not None:
+                stream.close()
+            reader.close()
+        if reader.error is not None:
+            raise reader.error
+
+    def _window_batches(self, window: List["_Recording"], chunk_size: int, batch_size: int, right: int, trim: bool):
+        """Features of a window of recordings -> [(corpus.Batch, feats (B, T, 80), lens (B,) int32)] in the order of
+        corpus.plan_window.  A row is the chunk's frames followed by zeros, as feats_batcher pads the last chunk."""
+        feats = [self._recording_feats(rec) for rec in window]
+        for rec in window:
+            rec.pcm = None
+        nbins = feats[0].shape[1]
+        for rec in window:
+            rec.chunks = rec.left = len(corpus.chunk_lengths(rec.frames, chunk_size))
+        plan = corpus.plan_window([rec.frames for rec in window], chunk_size, batch_size, right, trim)
+        starts = np.cumsum([0] + [f.shape[0] for f in feats])
+        flat = torch.cat(feats + [feats[0].new_zeros(1, nbins)])
+        zero_row = int(starts[-1])
+        out = []
+        for b in plan:
+            first = torch.tensor([int(starts[r]) + c * chunk_size for r, c in b.slots], dtype=torch.int64)
+            lens = torch.tensor(b.lens, dtype=torch.int32)
+            first_d = first.pin_memory().to(self.device, non_blocking=True)
+            lens_d = lens.to(torch.int64).pin_memory().to(self.device, non_blocking=True)
+            t = torch.arange(b.T, device=self.device)
+            rows = torch.where(t < lens_d[:, None], first_d[:, None] + t, zero_row)
+            out.append((b, flat.index_select(0, rows.reshape(-1)).view(len(b.slots), b.T, nbins), lens))
+        return out
 
     def transcribe(self, audio_file, mode: str = "ctc_prefix_beam_search", format: str = "txt",
                    verbatimicity: float = 1.0, chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
@@ -274,6 +384,89 @@ class ReverbASR:
             aligner.abort()
         return result, frames_to_ms(result.times, chunk_frames, chunk_size * self.input_frame_length,
                                     self.output_frame_length)
+
+
+def _check_fbank_conf(num_mel_bins, frame_length, frame_shift, dither=0.0, resample_rate=16000):
+    if num_mel_bins != 80 or frame_length != 25 or frame_shift != 10 or dither != 0.0 or resample_rate != 16000:
+        raise NotImplementedError("reverb_b200 fbank kernel is built for 80 bins / 25 ms / 10 ms / no dither @16 kHz")
+
+
+class _Recording:
+    """One recording of a transcribe_files call: channel 0 on the host, and its chunks' results as they arrive."""
+
+    def __init__(self, path, pcm: np.ndarray, sample_rate: int, frames: int):
+        self.path, self.pcm, self.sample_rate, self.frames = path, pcm, sample_rate, frames
+        self.chunks = self.left = 0
+        self.hyps: Dict[str, Dict[int, DecodeResult]] = {}
+
+
+def _name_file(e: BaseException, path) -> BaseException:
+    """`e`, or the same kind of exception with the file's name in front of its message."""
+    if str(path) in str(e):
+        return e
+    try:
+        named = type(e)(f"{path}: {e}")
+    except Exception:
+        return e
+    named.__cause__ = e
+    return named
+
+
+class _Reader:
+    """Reads and parses recordings on one background thread and hands them over in windows (corpus.WindowPacker),
+    one window ahead of the decoder.  Iteration ends before the first file that cannot be read; its error, naming
+    the file, is then in `error`."""
+
+    def __init__(self, asr: ReverbASR, files: list, budget: int):
+        self.error = None
+        self._q: queue.Queue = queue.Queue(maxsize=1)
+        self._stop = threading.Event()
+        self._thread = threading.Thread(target=self._run, args=(asr, files, budget), daemon=True,
+                                        name="reverb-reader")
+        self._thread.start()
+
+    def _put(self, item) -> bool:
+        while not self._stop.is_set():
+            try:
+                self._q.put(item, timeout=0.1)
+                return True
+            except queue.Full:
+                pass
+        return False
+
+    def _run(self, asr, files, budget):
+        packer = corpus.WindowPacker(budget)
+        try:
+            for f in files:
+                try:
+                    rec = asr._read_recording(f)
+                except Exception as e:
+                    window = packer.flush()
+                    if not window or self._put(window):
+                        self._put(_name_file(e, f))
+                    return
+                window = packer.add(rec.frames, rec)
+                if window and not self._put(window):
+                    return
+            window = packer.flush()
+            if window:
+                self._put(window)
+        finally:
+            self._put(None)
+
+    def __iter__(self):
+        while True:
+            item = self._q.get()
+            if item is None:
+                return
+            if isinstance(item, BaseException):
+                self.error = item
+                return
+            yield item
+
+    def close(self):
+        self._stop.set()
+        self._thread.join()
 
 
 def get_output(format: str, tokenizer, audio_name: str, hyps: List[DecodeResult], timings_adjustment_ms: int,
