@@ -38,10 +38,16 @@ __device__ __forceinline__ ArgMax warp_argmax(ArgMax a) {
 
 // One CTA per row.  Pass 1 stages the row in shared memory and keeps each thread's running (max, index); the 32
 // "lane-group" maxima (max over the threads with the same lane id, i.e. over the elements with index = lane mod 32)
-// are k <= 16 < 32 DISTINCT elements, so the k-th best of them is a lower bound of the row's k-th best: pass 2 (which
-// also accumulates sum exp(x - max)) collects the few elements that are not worse than it — typically k .. k+4 —
-// and one warp ranks those (value desc, index asc = torch.topk's order on ties).  If the candidate list overflows
-// (rows full of ties / -inf) the kernel falls back to k rounds of block arg-max.
+// are DISTINCT elements (a lane group without elements contributes (-inf, INT_MAX), which ranks below every element),
+// so the k-th best of them (k <= 16 < 32) is a lower bound of the row's k-th best: pass 2 (which also accumulates
+// sum exp(x - max)) collects the few elements that are not worse than it — typically k .. k+4 — and one warp ranks
+// those.  The kernel falls back to k rounds of block arg-max when that bound is -inf (fewer than k lane groups hold a
+// finite element) or when more than TOPK_CAP elements pass it (a lane group full of ties or high values).
+//
+// Order contract, on both paths: the k reported entries are the first k of a stable sort of the row by value,
+// descending — ties go to the lower index.  -inf entries are ordinary entries: a row with fewer than k finite entries
+// reports its finite ones first, then its lowest-index -inf columns in index order, with value -inf.  NaN entries
+// compare false and are never reported; if fewer than k entries are not NaN, the remaining slots get index 0.
 constexpr int TOPK_CAP = 64;
 
 __global__ void __launch_bounds__(256)
@@ -73,7 +79,7 @@ logsoftmax_topk_kernel(const float* __restrict__ logits, long long ld, int V, in
   if (lane == 0) s_red[warp] = m;
   if (threadIdx.x == 0) {
     s_ncand = 0;
-    s_thresh.v = -INFINITY;  // stays invalid when the group maxima are not all distinct (rows with < 32 entries)
+    s_thresh.v = -INFINITY;  // overwritten below by the k-th best lane-group maximum
     s_thresh.i = 0x7fffffff;
   }
   __syncthreads();
@@ -146,8 +152,10 @@ logsoftmax_topk_kernel(const float* __restrict__ logits, long long ld, int V, in
     return;
   }
   // fallback: k rounds of block arg-max over per-thread running maxima (ties -> lowest index); only the thread that
-  // owned the winner rescans its ~V/256 elements, one barrier per round
-  auto local_best = [&]() {
+  // owned the winner rescans its ~V/256 elements, one barrier per round.  The rescan keeps the elements strictly after
+  // the winner in (value desc, index asc) order: those are exactly the owner's elements not reported yet, so a
+  // reported -inf is never picked again and further -inf entries follow in index order.
+  auto local_best_after = [&](ArgMax prev) {
     ArgMax a;
     a.v = -INFINITY;
     a.i = 0x7fffffff;
@@ -155,7 +163,7 @@ logsoftmax_topk_kernel(const float* __restrict__ logits, long long ld, int V, in
       ArgMax e;
       e.v = s_row[i];
       e.i = i;
-      a = better(a, e);
+      if (e.v < prev.v || (e.v == prev.v && e.i > prev.i)) a = better(a, e);
     }
     return a;
   };
@@ -166,7 +174,7 @@ logsoftmax_topk_kernel(const float* __restrict__ logits, long long ld, int V, in
     ArgMax best = s_arg[r & 1][0];
 #pragma unroll
     for (int w = 1; w < 8; ++w) best = better(best, s_arg[r & 1][w]);
-    if (best.i == 0x7fffffff) {  // fewer than k finite entries left: report index 0 like the scan-based version
+    if (best.i == 0x7fffffff) {  // only NaN entries left (see the order contract above TOPK_CAP)
       if (threadIdx.x == 0) {
         topk_val[row * k + r] = (best.v - lse_shift) - logsum;
         topk_idx[row * k + r] = 0;
@@ -174,8 +182,7 @@ logsoftmax_topk_kernel(const float* __restrict__ logits, long long ld, int V, in
     } else if ((best.i & 255) == (int)threadIdx.x) {
       topk_val[row * k + r] = (best.v - lse_shift) - logsum;
       topk_idx[row * k + r] = best.i;
-      s_row[best.i] = -INFINITY;
-      mine = local_best();
+      mine = local_best_after(best);
     }
   }
 }
