@@ -139,6 +139,23 @@ struct Decoder {
   bool present = false;
 };
 
+// Row buffers of a decoder pass over R rows (grow-only): residual stream x (fp32), LayerNorm output n, projections qkv,
+// attention output att, FFN hidden h, LSL mix ybf, and the source-attention [k | v] of Mem encoder frames.  Every bf16
+// buffer is pm times as wide: the [hi | lo] pairs of the accurate mode.
+struct DecRows {
+  DevBuf x, n, qkv, att, h, ybf, kv;
+  int ensure(long long R, long long Mem, int d, int ffn, size_t pm) {
+    if (x.ensure((size_t)R * d * 4) || n.ensure((size_t)R * d * 2 * pm) || qkv.ensure((size_t)R * 3 * d * 2 * pm) ||
+        att.ensure((size_t)R * d * 2 * pm) || kv.ensure((size_t)Mem * 2 * d * 2 * pm) ||
+        h.ensure((size_t)R * ffn * 2 * pm) || ybf.ensure((size_t)R * d * 2 * pm))
+      return -1;
+    return 0;
+  }
+  void release() {
+    for (DevBuf* b : {&x, &n, &qkv, &att, &h, &ybf, &kv}) b->release();
+  }
+};
+
 }  // namespace rvb
 
 using namespace rvb;
@@ -168,8 +185,12 @@ struct rvb_model {
 
   // workspace (grow-only)
   DevBuf ws_c1, ws_c2, ws_x, ws_n, ws_h, ws_qkv, ws_att, ws_pw, ws_cm, ws_y, ws_ybf, ws_pe, ws_pall, ws_lens;
-  DevBuf ws_encbf, ws_logits, ws_dec[12], ws_search, ws_misc, ws_kpp, ws_cbias;
-  HostPinned pin_a, pin_b, pin_c, pin_d, pin_e;
+  DevBuf ws_encbf, ws_logits, ws_misc, ws_kpp, ws_cbias;
+  rvb::DecRows dec_rows;        // rows of the flat and prefix-tree decoder passes
+  DevBuf ws_lse;                // output layer: OUT_LSE partials + target logits
+  DevBuf ws_tree_idx, ws_edge_rows, ws_edge_scores;  // prefix-tree pass: node / edge indices, edge rows, edge scores
+  DevBuf ws_step_rows;          // full log_softmax rows of the last position (decoder_step_logp)
+  HostPinned pin_a, pin_b, pin_c;
   int pe_T = 0;
   int pall_T = 0;               // ws_pall holds linear_pos(pos_emb) for this many frames
   const void* pall_ptr = nullptr;
@@ -528,6 +549,88 @@ static int attn_impl() {
   return v;
 }
 
+// whether an attention of `dk`-wide heads runs on the wgmma kernel (bf16 mode only)
+static bool wgmma_attn(const rvb_model* m, int dk) { return !m->x3 && attn_impl() == 1 && dk == 64; }
+
+// One attention of the decoder.  q / k / v / out address column 0 of head 0, with their LOGICAL (plain bf16) row
+// strides; group g owns query rows [g*Tq, (g+1)*Tq) and key rows [g*Tk, (g+1)*Tk).  In the accurate mode every operand
+// is a [hi | lo] pair: physical stride 2 * ld, lo one logical width (ld) to the right.
+struct DecAttn {
+  const bf16* q = nullptr;
+  const bf16* k = nullptr;
+  const bf16* v = nullptr;
+  bf16* out = nullptr;
+  int ldq = 0, ldk = 0, ldv = 0, ldo = 0;
+  int groups = 0, Tq = 0, Tk = 0, H = 0, dk = 0;
+  float scale = 1.0f;
+  // the mask: key lengths (k_lens, per group), causal (with Tq == Tk, on top of k_lens), key bits (on top of causal,
+  // AttnTcArgs::key_bits) or key lists (AttnF32Args::key_list)
+  const int* k_lens = nullptr;
+  bool causal = false;
+  const uint32_t* key_bits = nullptr;
+  int bits_ld = 0;
+  const int* key_list = nullptr;
+  const int* key_list_len = nullptr;
+  int key_list_ld = 0;
+  bool f32 = false;  // the fp32 kernel in the bf16 mode too
+};
+
+// the kernel: fp32 in the accurate mode, when asked for, or for key lists; else wgmma (wgmma_attn); else mma.sync
+static int dec_attention(const rvb_model* m, const DecAttn& a, cudaStream_t stream) {
+  if (m->x3 || a.f32 || a.key_list) {
+    const int pm = m->pm(), lo = m->x3 ? 1 : 0;
+    AttnF32Args f;
+    f.q = a.q; f.k = a.k; f.v = a.v; f.out = a.out;
+    f.ldq = a.ldq * pm; f.ldk = a.ldk * pm; f.ldv = a.ldv * pm; f.ldo = a.ldo * pm;
+    f.q_lo = a.ldq * lo; f.k_lo = a.ldk * lo; f.v_lo = a.ldv * lo; f.o_lo = a.ldo * lo;
+    f.groups = a.groups; f.Tq = a.Tq; f.Tk = a.Tk; f.H = a.H; f.dk = a.dk;
+    f.k_lens = a.k_lens;
+    f.chunk = a.causal ? 1 : 0;  // chunk = 1, left < 0: causal
+    f.key_list = a.key_list; f.key_list_len = a.key_list_len; f.key_list_ld = a.key_list_ld;
+    return launch_attention_f32(f, stream);
+  }
+  if (wgmma_attn(m, a.dk)) {
+    AttnTcArgs t;
+    t.q = a.q; t.k = a.k; t.v = a.v; t.out = a.out;
+    t.ldq = a.ldq; t.ldk = a.ldk; t.ldv = a.ldv; t.ldo = a.ldo;
+    t.groups = a.groups; t.Tq = a.Tq; t.Tk = a.Tk; t.H = a.H; t.dk = a.dk;
+    t.k_lens = a.k_lens;
+    t.causal = a.causal;
+    t.key_bits = a.key_bits; t.bits_ld = a.bits_ld;
+    t.scale = a.scale;
+    return launch_attention_tc(t, stream);
+  }
+  RVB_REQUIRE(a.key_bits == nullptr, "decoder attention: key bit masks need the wgmma kernel");
+  AttnArgs s;
+  s.q = a.q; s.k = a.k; s.v = a.v; s.out = a.out;
+  s.ldq = a.ldq; s.ldk = a.ldk; s.ldv = a.ldv; s.ldo = a.ldo;
+  s.Bq = a.groups; s.Tq = a.Tq; s.Tk = a.Tk; s.H = a.H; s.dk = a.dk;
+  s.k_lens = a.k_lens;  // one query batch per key batch: the same key count as q_lens under the causal mask
+  s.causal = a.causal;
+  s.scale = a.scale;
+  return launch_attention(s, stream);
+}
+
+// source attention of Tq query rows per utterance (row stride d) over its Tp encoder frames, kv = [k | v] rows (2d)
+static DecAttn src_attention(bf16* q, const bf16* kv, bf16* out, int d, int B, int Tq, int Tp, int H,
+                             const int* d_enc_lens) {
+  DecAttn a;
+  a.q = q;
+  a.k = kv;
+  a.v = kv + d;
+  a.out = out;
+  a.ldq = a.ldo = d;
+  a.ldk = a.ldv = 2 * d;
+  a.groups = B;
+  a.Tq = Tq;
+  a.Tk = Tp;
+  a.H = H;
+  a.dk = d / H;
+  a.scale = 1.0f / sqrtf((float)a.dk);
+  a.k_lens = d_enc_lens;
+  return a;
+}
+
 // att_chunk > 0: bounded-context attention (add_optional_chunk_mask, utils/mask.py:126-197, with a fixed decoding chunk):
 // query frame i attends keys [max(0, (i/chunk - left) * chunk) (0 when left < 0), (i/chunk + 1) * chunk) & pad mask.
 static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat_lens, int B, int T,
@@ -575,7 +678,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
       m->ws_kpp.ensure((size_t)M * d * 2) ||
       m->ws_cbias.ensure(((size_t)B * H * Tp + (size_t)M * 2 * ((d / 2 + 127) / 128)) * 4))
     return -1;
-  const bool tc_attn = attn_impl() == 1 && dk == 64 && !x3;
+  const bool tc_attn = wgmma_attn(m, dk);
   if (!tc_attn && !x3 && attn_impl() == 1) {   // say so once: a d_k != 64 model runs the (slower) mma.sync attention
     static std::atomic<bool> warned{false};
     if (!warned.exchange(true))
@@ -796,17 +899,24 @@ __global__ void sub_column_kernel(float* x, long long ld, int rows, int col, flo
   if (r < rows) x[(long long)r * ld + col] -= v;
 }
 
+// the encoder output (Mem, d) fp32 as a GEMM operand in ws_encbf: bf16, or the [hi | lo] pair in the accurate mode
+static int enc_operand(rvb_model* m, const float* d_enc_out, long long Mem, bf16** out, cudaStream_t stream) {
+  const int d = m->cfg.d_model;
+  if (m->ws_encbf.ensure((size_t)Mem * d * 2 * m->pm())) return -1;
+  *out = m->ws_encbf.as<bf16>();
+  return m->x3 ? launch_f32_to_pair(d_enc_out, *out, Mem, d, stream) : launch_f32_to_bf16(d_enc_out, *out, Mem * d, stream);
+}
+
 static int ctc_topk(rvb_model* m, const float* d_enc_out, int B, int Tp, int k, float blank_penalty, int blank_id,
                     float* d_topk_val, int* d_topk_idx, float* d_logp, cudaStream_t stream) {
   const rvb_model_config& c = m->cfg;
   const long long M = (long long)B * Tp;
-  const int d = c.d_model, V = c.vocab;
+  const int V = c.vocab;
   const int ldv = (V + 3) & ~3;
-  if (m->ws_encbf.ensure((size_t)M * d * 2 * m->pm()) || m->ws_logits.ensure((size_t)M * ldv * 4)) return -1;
-  bf16* encbf = m->ws_encbf.as<bf16>();
+  if (m->ws_logits.ensure((size_t)M * ldv * 4)) return -1;
+  bf16* encbf;
   float* logits = m->ws_logits.as<float>();
-  if (m->x3 ? launch_f32_to_pair(d_enc_out, encbf, M, d, stream) : launch_f32_to_bf16(d_enc_out, encbf, M * d, stream))
-    return -1;
+  if (enc_operand(m, d_enc_out, M, &encbf, stream)) return -1;
   if (gemm(m, encbf, m->ctc, (int)M, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
   if (blank_penalty > 0.f) {
     sub_column_kernel<<<(int)((M + 255) / 256), 256, 0, stream>>>(logits, ldv, (int)M, blank_id, blank_penalty);
@@ -816,7 +926,104 @@ static int ctc_topk(rvb_model* m, const float* d_enc_out, int B, int Tp, int k, 
   return launch_logsoftmax_topk(logits, ldv, (int)M, V, k, d_topk_val, d_topk_idx, d_logp, 1, stream);
 }
 
-// One pass of a (LanguageSpecific)TransformerDecoder over R = S * Lp rows (S sequences of Lp positions).
+// The layers of a (LanguageSpecific)TransformerDecoder over the R rows of w.x, then after_norm -> w.n
+// (decoder_layer.py:95-110 / 286-301).  self_attn(l) attends from the [q | k | v] projection in w.qkv, src_attn(l) from
+// the q projection in w.qkv (row stride d) over the encoder output; both write w.att.
+template <class SelfAttn, class SrcAttn>
+static int decoder_layers(rvb_model* m, Decoder& D, DecRows& w, int R, SelfAttn self_attn, SrcAttn src_attn,
+                          cudaStream_t stream) {
+  const int d = m->cfg.d_model;
+  const bool x3 = m->x3;
+  float* x = w.x.as<float>();
+  bf16* n = w.n.as<bf16>();
+  bf16* qkv = w.qkv.as<bf16>();
+  bf16* att = w.att.as<bf16>();
+  bf16* h = w.h.as<bf16>();
+  bf16* ybf = w.ybf.as<bf16>();
+  for (size_t l = 0; l < D.layers.size(); ++l) {
+    DecLayer& Ld = D.layers[l];
+    // masked self-attention
+    if (launch_layernorm(x, Ld.n1.g, Ld.n1.b, Ld.eps, R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
+    if (gemm(m, n, Ld.qkv, R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
+    if (self_attn(l)) return -1;
+    if (gemm(m, att, Ld.so, R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
+    // source attention over the utterance's encoder output
+    if (launch_layernorm(x, Ld.n2.g, Ld.n2.b, Ld.eps, R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
+    if (gemm(m, n, Ld.cq, R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;  // q -> first d cols, ld = d
+    if (src_attn(l)) return -1;
+    if (gemm(m, att, Ld.co, R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
+    // feed forward (ReLU), language-specific mix first on LSL layers
+    if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
+    const bf16* ffn_in = n;
+    if (Ld.lsl) {
+      if (gemm(m, n, Ld.lang, R, ACT_NONE, OUT_BF16, ybf, 1.f, stream)) return -1;
+      ffn_in = ybf;
+    }
+    if (gemm(m, ffn_in, Ld.ff1, R, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
+    if (gemm(m, h, Ld.ff2, R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
+  }
+  return launch_layernorm(x, D.after.g, D.after.b, 1e-5f, R, d, n, nullptr, nullptr, 0, 0, stream, x3);
+}
+
+// Output layer: log-probability of the gather target of each of the M rows of A (gather < 0 -> 0) -> out (M)
+static int target_logp(rvb_model* m, const Decoder& D, const bf16* A, int M, const int* gather, float* out,
+                       cudaStream_t stream) {
+  const int V = m->cfg.vocab, ldv = (V + 3) & ~3;
+  if (get_gemm_impl() != 1 && V > 128) {
+    // log_softmax + gather fused into the output-layer GEMM: the (M, V) fp32 logits (4.2 GB at B = 64) are never
+    // written; the epilogue leaves per-slab (max, sum-exp) partials and the target logit, a small kernel merges them
+    const int slabs = lse_slabs(V);
+    if (m->ws_lse.ensure((size_t)M * slabs * sizeof(float2) + (size_t)M * sizeof(float))) return -1;
+    float2* part = m->ws_lse.as<float2>();
+    float* tgt = reinterpret_cast<float*>(part + (size_t)M * slabs);
+    GemmArgs g;
+    g.x3 = m->x3 ? 1 : 0;
+    g.A = A;
+    g.W = D.outl.w;
+    g.bias = D.outl.b;
+    g.M = M;
+    g.N = D.outl.N;
+    g.K = D.outl.K;
+    g.out_mode = OUT_LSE;
+    g.lse_gather = gather;
+    g.lse_part = part;
+    g.lse_tgt = tgt;
+    if (launch_gemm(g, stream)) return -1;
+    return launch_lse_merge(part, slabs, tgt, gather, M, out, stream);
+  }
+  if (m->ws_logits.ensure((size_t)M * ldv * 4)) return -1;
+  float* logits = m->ws_logits.as<float>();
+  if (gemm(m, A, D.outl, M, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
+  return launch_logsoftmax_gather(logits, ldv, M, V, gather, 1, out, stream);
+}
+
+// Output layer on the LAST of every Lp rows of n (S sequences): log_softmax + top-k -> val / idx (S, k), and the full
+// log_softmax rows -> logp (S, V) when given
+static int last_position_topk(rvb_model* m, const Decoder& D, const bf16* n, int S, int Lp, DevBuf& logits_buf, int k,
+                              float* val, int* idx, float* logp, cudaStream_t stream) {
+  const int d = m->cfg.d_model, V = m->cfg.vocab, ldv = (V + 3) & ~3, pm = m->pm();
+  if (logits_buf.ensure((size_t)S * ldv * 4)) return -1;
+  float* logits = logits_buf.as<float>();
+  // rows s*Lp + (Lp-1): the A operand is the strided view (S, d) with leading dimension Lp*d
+  GemmArgs g;
+  g.x3 = m->x3 ? 1 : 0;
+  g.A = n + (size_t)(Lp - 1) * d * pm;
+  g.lda = Lp * d * pm;
+  g.W = D.outl.w;
+  g.bias = D.outl.b;
+  g.M = S;
+  g.N = D.outl.N;
+  g.K = D.outl.K;
+  g.act = ACT_NONE;
+  g.out_mode = OUT_F32;
+  g.out = logits;
+  g.ldo = ldv;
+  g.alpha = 1.f;
+  if (launch_gemm(g, stream)) return -1;
+  return launch_logsoftmax_topk(logits, ldv, S, V, k, val, idx, logp, 1, stream);
+}
+
+// One pass of the decoder over R = S * Lp rows (S sequences of Lp positions).
 // Default: log-probability of the gather target at every position -> d_scores (attention rescoring).
 // step_k > 0 (autoregressive `attention` mode): only the LAST position of every sequence goes through the output
 // layer; log_softmax + top-step_k of it -> d_step_val / d_step_idx (S, step_k).
@@ -831,202 +1038,39 @@ static int decoder_pass(rvb_model* m, Decoder& D, const bf16* enc_bf, const int*
   const long long Mem = (long long)B * Tp;
   const int ldv = (V + 3) & ~3;
   RVB_REQUIRE(R < (1ll << 31) && R * ldv < (1ll << 40), "rescoring: too many hypothesis rows");
-  DevBuf* w = m->ws_dec;
-  const bool x3 = m->x3;
-  const size_t pm = (size_t)m->pm();
-  if (w[0].ensure((size_t)R * d * 4) || w[1].ensure((size_t)R * d * 2 * pm) || w[2].ensure((size_t)R * 3 * d * 2 * pm) ||
-      w[3].ensure((size_t)R * d * 2 * pm) || w[4].ensure((size_t)Mem * 2 * d * 2 * pm) ||
-      w[5].ensure((size_t)R * c.dec_ffn_dim * 2 * pm) || w[6].ensure((size_t)R * d * 2 * pm))
-    return -1;
-  float* x = w[0].as<float>();
-  bf16* n = w[1].as<bf16>();
-  bf16* qkv = w[2].as<bf16>();
-  bf16* att = w[3].as<bf16>();
-  bf16* kv = w[4].as<bf16>();
-  bf16* h = w[5].as<bf16>();
-  bf16* ybf = w[6].as<bf16>();
-  float* logits = nullptr;
-  const float scale = 1.0f / sqrtf((float)dk);
-  if (launch_embed_posenc(d_tokens, D.emb, S, Lp, d, x, stream)) return -1;
-  for (size_t l = 0; l < D.layers.size(); ++l) {
-    DecLayer& Ld = D.layers[l];
-    // masked self-attention (decoder_layer.py:95-110 / 286-301)
-    if (launch_layernorm(x, Ld.n1.g, Ld.n1.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.qkv, (int)R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
-    if (x3) {
-      AttnF32Args a;  // one group per hypothesis, causal, keys beyond the hypothesis length masked
-      a.q = qkv;
-      a.k = qkv + d;
-      a.v = qkv + 2 * d;
-      a.out = att;
-      a.ldq = a.ldk = a.ldv = 6 * d;
-      a.q_lo = a.k_lo = a.v_lo = 3 * d;
-      a.ldo = 2 * d;
-      a.o_lo = d;
-      a.groups = S;
-      a.Tq = Lp;
-      a.Tk = Lp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_seq_lens;
-      a.chunk = 1;
-      a.left = -1;
-      if (launch_attention_f32(a, stream)) return -1;
-    } else if (attn_impl() == 1 && dk == 64) {
-      AttnTcArgs a;  // one group per hypothesis, causal, keys beyond the hypothesis length masked
-      a.q = qkv;
-      a.k = qkv + d;
-      a.v = qkv + 2 * d;
-      a.out = att;
-      a.ldq = a.ldk = a.ldv = 3 * d;
-      a.ldo = d;
-      a.groups = S;
-      a.Tq = Lp;
-      a.Tk = Lp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_seq_lens;
-      a.causal = 1;
-      a.scale = scale;
-      if (launch_attention_tc(a, stream)) return -1;
-    } else {
-      AttnArgs a;
-      a.q = qkv;
-      a.k = qkv + d;
-      a.v = qkv + 2 * d;
-      a.out = att;
-      a.ldq = a.ldk = a.ldv = 3 * d;
-      a.ldo = d;
-      a.Bq = S;
-      a.Tq = Lp;
-      a.Tk = Lp;
-      a.H = H;
-      a.dk = dk;
-      a.q_lens = d_seq_lens;
-      a.causal = 1;
-      a.scale = scale;
-      if (launch_attention(a, stream)) return -1;
-    }
-    if (gemm(m, att, Ld.so, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    // source attention over the utterance's encoder output, K/V projected ONCE per utterance
-    if (launch_layernorm(x, Ld.n2.g, Ld.n2.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.cq, (int)R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;  // q -> first d cols, ld = d
-    if (gemm(m, enc_bf, Ld.ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
-    if (x3) {
-      AttnF32Args a;  // one group per utterance: its N hypotheses share the keys
-      a.q = qkv;
-      a.k = kv;
-      a.v = kv + d;
-      a.out = att;
-      a.ldq = 2 * d;
-      a.q_lo = d;
-      a.ldk = a.ldv = 4 * d;
-      a.k_lo = a.v_lo = 2 * d;
-      a.ldo = 2 * d;
-      a.o_lo = d;
-      a.groups = B;
-      a.Tq = N * Lp;
-      a.Tk = Tp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_enc_lens;
-      if (launch_attention_f32(a, stream)) return -1;
-    } else if (attn_impl() == 1 && dk == 64) {
-      // the N hypotheses of an utterance share its keys: one group per utterance with N * Lp query rows
-      AttnTcArgs a;
-      a.q = qkv;
-      a.k = kv;
-      a.v = kv + d;
-      a.out = att;
-      a.ldq = d;
-      a.ldk = a.ldv = 2 * d;
-      a.ldo = d;
-      a.groups = B;
-      a.Tq = N * Lp;
-      a.Tk = Tp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_enc_lens;
-      a.scale = scale;
-      if (launch_attention_tc(a, stream)) return -1;
-    } else {
-      AttnArgs a;
-      a.q = qkv;
-      a.k = kv;
-      a.v = kv + d;
-      a.out = att;
-      a.ldq = d;
-      a.ldk = a.ldv = 2 * d;
-      a.ldo = d;
-      a.Bq = S;
-      a.Tq = Lp;
-      a.Tk = Tp;
-      a.H = H;
-      a.dk = dk;
-      a.q_per_kv = N;
-      a.k_lens = d_enc_lens;
-      a.scale = scale;
-      if (launch_attention(a, stream)) return -1;
-    }
-    if (gemm(m, att, Ld.co, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    // feed forward (ReLU), language-specific mix first on LSL layers
-    if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    const bf16* ffn_in = n;
-    if (Ld.lsl) {
-      if (gemm(m, n, Ld.lang, (int)R, ACT_NONE, OUT_BF16, ybf, 1.f, stream)) return -1;
-      ffn_in = ybf;
-    }
-    if (gemm(m, ffn_in, Ld.ff1, (int)R, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
-    if (gemm(m, h, Ld.ff2, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-  }
-  if (launch_layernorm(x, D.after.g, D.after.b, 1e-5f, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-  if (step_k > 0) {
-    // rows s*Lp + (Lp-1): the A operand is the strided view (S, d) with leading dimension Lp*d
-    if (m->ws_logits.ensure((size_t)S * ldv * 4)) return -1;
-    logits = m->ws_logits.as<float>();
-    GemmArgs g;
-    g.x3 = x3 ? 1 : 0;
-    g.A = n + (size_t)(Lp - 1) * d * pm;
-    g.lda = Lp * d * (int)pm;
-    g.W = D.outl.w;
-    g.bias = D.outl.b;
-    g.M = S;
-    g.N = D.outl.N;
-    g.K = D.outl.K;
-    g.act = ACT_NONE;
-    g.out_mode = OUT_F32;
-    g.out = logits;
-    g.ldo = ldv;
-    g.alpha = 1.f;
-    if (launch_gemm(g, stream)) return -1;
-    return launch_logsoftmax_topk(logits, ldv, S, V, step_k, d_step_val, d_step_idx, d_step_logp, 1, stream);
-  }
-  if (get_gemm_impl() != 1 && V > 128) {
-    // log_softmax + gather fused into the output-layer GEMM: the (R, V) fp32 logits (4.2 GB at B = 64) are never
-    // written; the epilogue leaves per-slab (max, sum-exp) partials and the target logit, a small kernel merges them
-    const int slabs = lse_slabs(V);
-    if (w[7].ensure((size_t)R * slabs * sizeof(float2) + (size_t)R * sizeof(float))) return -1;
-    float2* part = w[7].as<float2>();
-    float* tgt = reinterpret_cast<float*>(part + (size_t)R * slabs);
-    GemmArgs g;
-    g.x3 = x3 ? 1 : 0;
-    g.A = n;
-    g.W = D.outl.w;
-    g.bias = D.outl.b;
-    g.M = (int)R;
-    g.N = D.outl.N;
-    g.K = D.outl.K;
-    g.out_mode = OUT_LSE;
-    g.lse_gather = d_gather;
-    g.lse_part = part;
-    g.lse_tgt = tgt;
-    if (launch_gemm(g, stream)) return -1;
-    return launch_lse_merge(part, slabs, tgt, d_gather, (int)R, d_scores, stream);
-  }
-  if (m->ws_logits.ensure((size_t)R * ldv * 4)) return -1;
-  logits = m->ws_logits.as<float>();
-  if (gemm(m, n, D.outl, (int)R, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
-  return launch_logsoftmax_gather(logits, ldv, (int)R, V, d_gather, 1, d_scores, stream);
+  DecRows& w = m->dec_rows;
+  if (w.ensure(R, Mem, d, c.dec_ffn_dim, m->pm())) return -1;
+  bf16* qkv = w.qkv.as<bf16>();
+  bf16* att = w.att.as<bf16>();
+  bf16* kv = w.kv.as<bf16>();
+  if (launch_embed_posenc(d_tokens, D.emb, S, Lp, d, w.x.as<float>(), stream)) return -1;
+  auto self_attn = [&](size_t) {
+    DecAttn a;  // one group per hypothesis, causal, keys beyond the hypothesis length masked
+    a.q = qkv;
+    a.k = qkv + d;
+    a.v = qkv + 2 * d;
+    a.out = att;
+    a.ldq = a.ldk = a.ldv = 3 * d;
+    a.ldo = d;
+    a.groups = S;
+    a.Tq = a.Tk = Lp;
+    a.H = H;
+    a.dk = dk;
+    a.scale = 1.0f / sqrtf((float)dk);
+    a.k_lens = d_seq_lens;
+    a.causal = true;
+    return dec_attention(m, a, stream);
+  };
+  auto src_attn = [&](size_t l) {
+    // K/V projected ONCE per utterance; its N hypotheses share the keys: one group of N * Lp query rows per utterance
+    if (gemm(m, enc_bf, D.layers[l].ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
+    return dec_attention(m, src_attention(qkv, kv, att, d, B, N * Lp, Tp, H, d_enc_lens), stream);
+  };
+  if (decoder_layers(m, D, w, (int)R, self_attn, src_attn, stream)) return -1;
+  if (step_k > 0)
+    return last_position_topk(m, D, w.n.as<bf16>(), S, Lp, m->ws_logits, step_k, d_step_val, d_step_idx, d_step_logp,
+                              stream);
+  return target_logp(m, D, w.n.as<bf16>(), (int)R, d_gather, d_scores, stream);
 }
 
 // One step of the autoregressive `attention` decode mode (decoder.forward_one_step + logp.topk, search.py:302-306):
@@ -1038,15 +1082,14 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   const rvb_model_config& c = m->cfg;
   RVB_REQUIRE(m->finalized && m->dec_l.present, "decoder_step_topk: model has no decoder");
   RVB_REQUIRE(L >= 1 && k >= 1 && k <= 16 && k <= c.vocab, "decoder_step_topk: bad L=%d / k=%d", L, k);
-  const int d = c.d_model, S = B * N;
+  const int S = B * N;
   const long long R = (long long)S * L, Mem = (long long)B * Tp;
   if (fold_lang(m, h_cat, n_cat, stream)) return -1;
   const size_t ints = (size_t)R + S + B;
   const size_t out_bytes = (size_t)S * k * (sizeof(float) + sizeof(int));
   const size_t row_bytes = h_logp ? (size_t)S * c.vocab * sizeof(float) : 0;
   if (m->pin_b.ensure(ints * sizeof(int)) || m->ws_misc.ensure(ints * sizeof(int) + out_bytes) ||
-      m->pin_c.ensure(out_bytes + row_bytes) || m->ws_encbf.ensure((size_t)Mem * d * 2 * m->pm()) ||
-      (h_logp && m->ws_dec[8].ensure(row_bytes)))
+      m->pin_c.ensure(out_bytes + row_bytes) || (h_logp && m->ws_step_rows.ensure(row_bytes)))
     return -1;
   int* hp = m->pin_b.as<int>();
   for (long long r = 0; r < R; ++r) {
@@ -1059,10 +1102,9 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   RVB_CHECK_CUDA(cudaMemcpyAsync(dp, hp, ints * sizeof(int), cudaMemcpyHostToDevice, stream));
   float* d_val = reinterpret_cast<float*>(dp + ints);
   int* d_idx = reinterpret_cast<int*>(d_val + (size_t)S * k);
-  bf16* encbf = m->ws_encbf.as<bf16>();
-  if (m->x3 ? launch_f32_to_pair(d_enc_out, encbf, Mem, d, stream) : launch_f32_to_bf16(d_enc_out, encbf, Mem * d, stream))
-    return -1;
-  float* d_rows = h_logp ? m->ws_dec[8].as<float>() : nullptr;
+  bf16* encbf;
+  if (enc_operand(m, d_enc_out, Mem, &encbf, stream)) return -1;
+  float* d_rows = h_logp ? m->ws_step_rows.as<float>() : nullptr;
   if (decoder_pass(m, m->dec_l, encbf, dp + R + S, B, Tp, N, L, dp, dp + R, nullptr, nullptr, stream, k, d_val, d_idx,
                    d_rows))
     return -1;
@@ -1089,12 +1131,14 @@ struct DecCache {
   bool flip = false;
   std::vector<DevBuf> self_a, self_b, cross;  // per layer
   DevBuf ints;   // enc lens (B) | key counts (S) | tokens (S) | parents (S)
-  DevBuf x, n, qkv, att, h, ybf, logits, outv;
+  DecRows rows;  // S rows (kv unused: `cross` holds the source-attention keys / values)
+  DevBuf logits, outv;
   HostPinned pin;
   void release() {
     for (auto* v : {&self_a, &self_b, &cross})
       for (auto& b : *v) b.release();
-    for (DevBuf* b : {&ints, &x, &n, &qkv, &att, &h, &ybf, &logits, &outv}) b->release();
+    for (DevBuf* b : {&ints, &logits, &outv}) b->release();
+    rows.release();
     pin.release();
   }
 };
@@ -1119,19 +1163,15 @@ static int decoder_cache_begin(rvb_model* m, const float* d_enc_out, const int* 
         dc.cross[l].ensure((size_t)Mem * kvw * 2))
       return -1;
   const int ldv = (c.vocab + 3) & ~3;
-  if (dc.ints.ensure(sizeof(int) * ((size_t)B + 3 * S)) || dc.x.ensure((size_t)S * d * 4) ||
-      dc.n.ensure((size_t)S * d * 2 * pm) || dc.qkv.ensure((size_t)S * 3 * d * 2 * pm) ||
-      dc.att.ensure((size_t)S * d * 2 * pm) || dc.h.ensure((size_t)S * c.dec_ffn_dim * 2 * pm) ||
-      dc.ybf.ensure((size_t)S * d * 2 * pm) || dc.logits.ensure((size_t)S * ldv * 4) ||
-      dc.outv.ensure((size_t)S * 16 * 8) || dc.pin.ensure(sizeof(int) * ((size_t)B + 2 * S) + (size_t)S * 16 * 8) ||
-      m->ws_encbf.ensure((size_t)Mem * d * 2 * pm))
+  if (dc.ints.ensure(sizeof(int) * ((size_t)B + 3 * S)) || dc.rows.ensure(S, 0, d, c.dec_ffn_dim, pm) ||
+      dc.logits.ensure((size_t)S * ldv * 4) || dc.outv.ensure((size_t)S * 16 * 8) ||
+      dc.pin.ensure(sizeof(int) * ((size_t)B + 2 * S) + (size_t)S * 16 * 8))
     return -1;
   int* hp = dc.pin.as<int>();
   memcpy(hp, h_enc_lens, sizeof(int) * B);
   RVB_CHECK_CUDA(cudaMemcpyAsync(dc.ints.p, hp, sizeof(int) * B, cudaMemcpyHostToDevice, stream));
-  bf16* encbf = m->ws_encbf.as<bf16>();
-  if (m->x3 ? launch_f32_to_pair(d_enc_out, encbf, Mem, d, stream) : launch_f32_to_bf16(d_enc_out, encbf, Mem * d, stream))
-    return -1;
+  bf16* encbf;
+  if (enc_operand(m, d_enc_out, Mem, &encbf, stream)) return -1;
   for (size_t l = 0; l < nl; ++l)   // source-attention keys / values: once per utterance, not once per step
     if (gemm(m, encbf, D.layers[l].ckv, (int)Mem, ACT_NONE, OUT_BF16, dc.cross[l].p, 1.f, stream)) return -1;
   return 0;
@@ -1145,7 +1185,7 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
   RVB_REQUIRE(m->dcache != nullptr && m->dcache->S > 0, "decoder_cache_step: call decoder_cache_begin first");
   DecCache& dc = *m->dcache;
   Decoder& D = m->dec_l;
-  const int d = c.d_model, H = c.dec_heads, dk = d / H, V = c.vocab, S = dc.S, B = dc.B, N = dc.N, pos = dc.step;
+  const int d = c.d_model, H = c.dec_heads, V = c.vocab, S = dc.S, B = dc.B, N = dc.N, pos = dc.step;
   RVB_REQUIRE(pos < dc.Lcap, "decoder_cache_step: step %d exceeds the cache capacity %d", pos, dc.Lcap);
   RVB_REQUIRE(k >= 1 && k <= 16 && k <= V, "decoder_cache_step: bad k=%d", k);
   const bool x3 = m->x3;
@@ -1167,88 +1207,45 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
   std::vector<DevBuf>& cur = dc.flip ? dc.self_b : dc.self_a;
   std::vector<DevBuf>& nxt = dc.flip ? dc.self_a : dc.self_b;
   const bool reorder = h_parents != nullptr && pos > 0;
-  float* x = dc.x.as<float>();
-  bf16* n = dc.n.as<bf16>();
-  bf16* qkv = dc.qkv.as<bf16>();
-  bf16* att = dc.att.as<bf16>();
-  bf16* h = dc.h.as<bf16>();
-  bf16* ybf = dc.ybf.as<bf16>();
-  if (launch_embed_posenc(d_tok, D.emb, S, 1, d, x, stream, pos)) return -1;
-  for (size_t l = 0; l < D.layers.size(); ++l) {
-    DecLayer& Ld = D.layers[l];
+  bf16* qkv = dc.rows.qkv.as<bf16>();
+  bf16* att = dc.rows.att.as<bf16>();
+  if (launch_embed_posenc(d_tok, D.emb, S, 1, d, dc.rows.x.as<float>(), stream, pos)) return -1;
+  auto self_attn = [&](size_t l) {
     bf16* cache = cur[l].as<bf16>();
     if (reorder) {  // the hypotheses were re-ranked: their histories follow (search.py:341-346)
       if (launch_kv_reorder(cache, nxt[l].as<bf16>(), d_par, S, dc.Lcap, pos, kvw, stream)) return -1;
       cache = nxt[l].as<bf16>();
     }
-    // self-attention of the new position over its own history
-    if (launch_layernorm(x, Ld.n1.g, Ld.n1.b, Ld.eps, S, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.qkv, S, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
     // cache row = [k | v] = columns [d, 3d) of the projection (and their lo halves at +3d in the pair layout)
     if (launch_kv_append(qkv, 3 * d * pm, d, cache, S, dc.Lcap, pos, 2 * d, kvw, stream)) return -1;
     if (x3 && launch_kv_append(qkv, 3 * d * pm, 3 * d + d, cache + 2 * d, S, dc.Lcap, pos, 2 * d, kvw, stream)) return -1;
-    {
-      AttnF32Args a;
-      a.q = qkv;
-      a.ldq = 3 * d * pm;
-      a.q_lo = x3 ? 3 * d : 0;
-      a.k = cache;
-      a.v = cache + d;
-      a.ldk = a.ldv = kvw;
-      a.k_lo = a.v_lo = x3 ? 2 * d : 0;
-      a.out = att;
-      a.ldo = d * pm;
-      a.o_lo = x3 ? d : 0;
-      a.groups = S;
-      a.Tq = 1;
-      a.Tk = dc.Lcap;      // group stride; the visible keys are [0, pos]
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_klen;
-      if (launch_attention_f32(a, stream)) return -1;
-    }
-    if (gemm(m, att, Ld.so, S, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    // source attention over the utterance's encoder output
-    if (launch_layernorm(x, Ld.n2.g, Ld.n2.b, Ld.eps, S, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.cq, S, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
-    {
-      AttnF32Args a;
-      a.q = qkv;
-      a.ldq = d * pm;
-      a.q_lo = x3 ? d : 0;
-      a.k = dc.cross[l].as<bf16>();
-      a.v = a.k + d;
-      a.ldk = a.ldv = kvw;
-      a.k_lo = a.v_lo = x3 ? 2 * d : 0;
-      a.out = att;
-      a.ldo = d * pm;
-      a.o_lo = x3 ? d : 0;
-      a.groups = B;
-      a.Tq = N;
-      a.Tk = dc.Tp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_elen;
-      if (launch_attention_f32(a, stream)) return -1;
-    }
-    if (gemm(m, att, Ld.co, S, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, S, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    const bf16* ffn_in = n;
-    if (Ld.lsl) {
-      if (gemm(m, n, Ld.lang, S, ACT_NONE, OUT_BF16, ybf, 1.f, stream)) return -1;
-      ffn_in = ybf;
-    }
-    if (gemm(m, ffn_in, Ld.ff1, S, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
-    if (gemm(m, h, Ld.ff2, S, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-  }
+    DecAttn a;  // the new position over its own history
+    a.q = qkv;
+    a.k = cache;
+    a.v = cache + d;
+    a.out = att;
+    a.ldq = 3 * d;
+    a.ldk = a.ldv = 2 * d;
+    a.ldo = d;
+    a.groups = S;
+    a.Tq = 1;
+    a.Tk = dc.Lcap;  // group stride; the visible keys are [0, pos]
+    a.H = H;
+    a.dk = d / H;
+    a.k_lens = d_klen;
+    a.f32 = true;
+    return dec_attention(m, a, stream);
+  };
+  auto src_attn = [&](size_t l) {
+    DecAttn a = src_attention(qkv, dc.cross[l].as<bf16>(), att, d, B, N, dc.Tp, H, d_elen);
+    a.f32 = true;
+    return dec_attention(m, a, stream);
+  };
+  if (decoder_layers(m, D, dc.rows, S, self_attn, src_attn, stream)) return -1;
   if (reorder) dc.flip = !dc.flip;
-  if (launch_layernorm(x, D.after.g, D.after.b, 1e-5f, S, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-  const int ldv = (V + 3) & ~3;
-  float* logits = dc.logits.as<float>();
-  if (gemm(m, n, D.outl, S, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
   float* d_val = dc.outv.as<float>();
   int* d_idx = reinterpret_cast<int*>(d_val + (size_t)S * k);
-  if (launch_logsoftmax_topk(logits, ldv, S, V, k, d_val, d_idx, nullptr, 1, stream)) return -1;
+  if (last_position_topk(m, D, dc.rows.n.as<bf16>(), S, 1, dc.logits, k, d_val, d_idx, nullptr, stream)) return -1;
   char* hout = reinterpret_cast<char*>(dc.pin.as<int>() + B + 2 * S);
   const size_t out_bytes = (size_t)S * k * (sizeof(float) + sizeof(int));
   RVB_CHECK_CUDA(cudaMemcpyAsync(hout, d_val, out_bytes, cudaMemcpyDeviceToHost, stream));
@@ -1282,31 +1279,23 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
                              int Lp, int P, const TrieView& tv, const int* d_olen, const int* d_nhyp, float* d_scores,
                              cudaStream_t stream) {
   const rvb_model_config& c = m->cfg;
-  const int d = c.d_model, H = c.dec_heads, dk = d / H, V = c.vocab;
+  const int d = c.d_model, H = c.dec_heads, dk = d / H;
   const long long R = (long long)B * P, E = (long long)B * (P + N), Mem = (long long)B * Tp;
   const long long S = (long long)B * N;
-  const bool x3 = m->x3;
   const size_t pm = (size_t)m->pm();
-  const int ldv = (V + 3) & ~3;
-  DevBuf* w = m->ws_dec;
-  // bf16 mode: self-attention of the tree on the wgmma kernel (dense over the utterance's P node slots, causal tile
-  // range — a parent always precedes its children — plus an ancestor bit mask); accurate mode: fp32 over ancestor lists
-  const bool tc_self = !x3 && attn_impl() == 1 && dk == 64 && !(getenv("RVB_TRIE_ATTN") && strcmp(getenv("RVB_TRIE_ATTN"), "list") == 0);
+  // self-attention of the tree on the wgmma kernel: dense over the utterance's P node slots, causal tile range (a
+  // parent always precedes its children) plus an ancestor bit mask; otherwise fp32 over ancestor lists
+  const bool tc_self = wgmma_attn(m, dk) && !(getenv("RVB_TRIE_ATTN") && strcmp(getenv("RVB_TRIE_ATTN"), "list") == 0);
   const int bits_ld = 2 * ((P + 63) / 64);
   const size_t n_int = (size_t)R * 3 + (size_t)R * Lp + (size_t)E * 2 + (size_t)S * Lp + (tc_self ? (size_t)R * bits_ld : 0);
-  if (w[0].ensure((size_t)R * d * 4) || w[1].ensure((size_t)R * d * 2 * pm) || w[2].ensure((size_t)R * 3 * d * 2 * pm) ||
-      w[3].ensure((size_t)R * d * 2 * pm) || w[4].ensure((size_t)Mem * 2 * d * 2 * pm) ||
-      w[5].ensure((size_t)R * c.dec_ffn_dim * 2 * pm) || w[6].ensure((size_t)R * d * 2 * pm) ||
-      w[9].ensure(n_int * sizeof(int)) || w[10].ensure((size_t)E * d * 2 * pm) || w[11].ensure((size_t)E * sizeof(float)))
+  DecRows& w = m->dec_rows;
+  if (w.ensure(R, Mem, d, c.dec_ffn_dim, pm) || m->ws_tree_idx.ensure(n_int * sizeof(int)) ||
+      m->ws_edge_rows.ensure((size_t)E * d * 2 * pm) || m->ws_edge_scores.ensure((size_t)E * sizeof(float)))
     return -1;
-  float* x = w[0].as<float>();
-  bf16* n = w[1].as<bf16>();
-  bf16* qkv = w[2].as<bf16>();
-  bf16* att = w[3].as<bf16>();
-  bf16* kv = w[4].as<bf16>();
-  bf16* h = w[5].as<bf16>();
-  bf16* ybf = w[6].as<bf16>();
-  int* tok_in = w[9].as<int>();
+  bf16* qkv = w.qkv.as<bf16>();
+  bf16* att = w.att.as<bf16>();
+  bf16* kv = w.kv.as<bf16>();
+  int* tok_in = m->ws_tree_idx.as<int>();
   int* pos = tok_in + R;
   int* alen = pos + R;
   int* anc = alen + R;
@@ -1314,135 +1303,47 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
   int* tgt = src + E;
   int* smap = tgt + E;
   uint32_t* anc_bits = tc_self ? reinterpret_cast<uint32_t*>(smap + (size_t)S * Lp) : nullptr;
-  bf16* a_out = w[10].as<bf16>();
-  float* e_sc = w[11].as<float>();
+  bf16* a_out = m->ws_edge_rows.as<bf16>();
+  float* e_sc = m->ws_edge_scores.as<float>();
   if (launch_trie_inputs(tv.node_of, tv.nstride, tv.node_tok, tv.node_par, tv.node_dep, tv.cap, tv.n_nodes, d_olen, d_nhyp,
                          B, N, P, Lp, eos_id(c), tok_in, pos, anc, alen, src, tgt, smap, stream, anc_bits, bits_ld))
     return -1;
-  if (launch_embed_posenc_rows(tok_in, pos, D.emb, (int)R, d, x, stream)) return -1;
-  for (size_t l = 0; l < D.layers.size(); ++l) {
-    DecLayer& Ld = D.layers[l];
-    // self-attention of every node over its ancestors (= the causal mask of the flat layout)
-    if (launch_layernorm(x, Ld.n1.g, Ld.n1.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.qkv, (int)R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
+  if (launch_embed_posenc_rows(tok_in, pos, D.emb, (int)R, d, w.x.as<float>(), stream)) return -1;
+  auto self_attn = [&](size_t) {
+    DecAttn a;  // every node over its ancestors (= the causal mask of the flat layout)
+    a.q = qkv;
+    a.k = qkv + d;
+    a.v = qkv + 2 * d;
+    a.out = att;
+    a.ldq = a.ldk = a.ldv = 3 * d;
+    a.ldo = d;
+    a.H = H;
+    a.dk = dk;
+    a.scale = 1.0f / sqrtf((float)dk);
     if (tc_self) {
-      AttnTcArgs a;
-      a.q = qkv;
-      a.k = qkv + d;
-      a.v = qkv + 2 * d;
-      a.out = att;
-      a.ldq = a.ldk = a.ldv = 3 * d;
-      a.ldo = d;
       a.groups = B;
-      a.Tq = P;
-      a.Tk = P;
-      a.H = H;
-      a.dk = dk;
-      a.causal = 1;
+      a.Tq = a.Tk = P;
+      a.causal = true;
       a.key_bits = anc_bits;
       a.bits_ld = bits_ld;
-      a.scale = 1.0f / sqrtf((float)dk);
-      if (launch_attention_tc(a, stream)) return -1;
     } else {
-      AttnF32Args a;
-      a.q = qkv;
-      a.k = qkv + d;
-      a.v = qkv + 2 * d;
-      a.out = att;
-      a.ldq = a.ldk = a.ldv = 3 * d * (int)pm;
-      a.q_lo = a.k_lo = a.v_lo = x3 ? 3 * d : 0;
-      a.ldo = d * (int)pm;
-      a.o_lo = x3 ? d : 0;
       a.groups = 1;
       a.Tq = (int)R;
       a.Tk = Lp;
-      a.H = H;
-      a.dk = dk;
       a.key_list = anc;
       a.key_list_len = alen;
       a.key_list_ld = Lp;
-      if (launch_attention_f32(a, stream)) return -1;
     }
-    if (gemm(m, att, Ld.so, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    // source attention over the utterance's encoder output (K/V projected once per utterance)
-    if (launch_layernorm(x, Ld.n2.g, Ld.n2.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    if (gemm(m, n, Ld.cq, (int)R, ACT_NONE, OUT_BF16, qkv, 1.f, stream)) return -1;
-    if (gemm(m, enc_bf, Ld.ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
-    if (!x3 && attn_impl() == 1 && dk == 64) {
-      AttnTcArgs a;
-      a.q = qkv;
-      a.k = kv;
-      a.v = kv + d;
-      a.out = att;
-      a.ldq = d;
-      a.ldk = a.ldv = 2 * d;
-      a.ldo = d;
-      a.groups = B;
-      a.Tq = P;
-      a.Tk = Tp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_enc_lens;
-      a.scale = 1.0f / sqrtf((float)dk);
-      if (launch_attention_tc(a, stream)) return -1;
-    } else {
-      AttnF32Args a;
-      a.q = qkv;
-      a.k = kv;
-      a.v = kv + d;
-      a.out = att;
-      a.ldq = d * (int)pm;
-      a.q_lo = x3 ? d : 0;
-      a.ldk = a.ldv = 2 * d * (int)pm;
-      a.k_lo = a.v_lo = x3 ? 2 * d : 0;
-      a.ldo = d * (int)pm;
-      a.o_lo = x3 ? d : 0;
-      a.groups = B;
-      a.Tq = P;
-      a.Tk = Tp;
-      a.H = H;
-      a.dk = dk;
-      a.k_lens = d_enc_lens;
-      if (launch_attention_f32(a, stream)) return -1;
-    }
-    if (gemm(m, att, Ld.co, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-    if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
-    const bf16* ffn_in = n;
-    if (Ld.lsl) {
-      if (gemm(m, n, Ld.lang, (int)R, ACT_NONE, OUT_BF16, ybf, 1.f, stream)) return -1;
-      ffn_in = ybf;
-    }
-    if (gemm(m, ffn_in, Ld.ff1, (int)R, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
-    if (gemm(m, h, Ld.ff2, (int)R, ACT_NONE, OUT_RESID_F32, x, 1.f, stream)) return -1;
-  }
-  if (launch_layernorm(x, D.after.g, D.after.b, 1e-5f, (int)R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
+    return dec_attention(m, a, stream);
+  };
+  auto src_attn = [&](size_t l) {  // K/V projected once per utterance
+    if (gemm(m, enc_bf, D.layers[l].ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
+    return dec_attention(m, src_attention(qkv, kv, att, d, B, P, Tp, H, d_enc_lens), stream);
+  };
+  if (decoder_layers(m, D, w, (int)R, self_attn, src_attn, stream)) return -1;
   // output layer on one row per EDGE of the tree (+ one per hypothesis end): hidden state of the edge's source node
-  if (launch_gather_rows(n, src, a_out, (int)E, d * (int)pm, stream)) return -1;
-  if (get_gemm_impl() != 1 && V > 128) {
-    const int slabs = lse_slabs(V);
-    if (w[7].ensure((size_t)E * slabs * sizeof(float2) + (size_t)E * sizeof(float))) return -1;
-    float2* part = w[7].as<float2>();
-    float* tg = reinterpret_cast<float*>(part + (size_t)E * slabs);
-    GemmArgs g;
-    g.x3 = x3 ? 1 : 0;
-    g.A = a_out;
-    g.W = D.outl.w;
-    g.bias = D.outl.b;
-    g.M = (int)E;
-    g.N = D.outl.N;
-    g.K = D.outl.K;
-    g.out_mode = OUT_LSE;
-    g.lse_gather = tgt;
-    g.lse_part = part;
-    g.lse_tgt = tg;
-    if (launch_gemm(g, stream)) return -1;
-    if (launch_lse_merge(part, slabs, tg, tgt, (int)E, e_sc, stream)) return -1;
-  } else {
-    if (m->ws_logits.ensure((size_t)E * ldv * 4)) return -1;
-    float* logits = m->ws_logits.as<float>();
-    if (gemm(m, a_out, D.outl, (int)E, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
-    if (launch_logsoftmax_gather(logits, ldv, (int)E, V, tgt, 1, e_sc, stream)) return -1;
-  }
+  if (launch_gather_rows(w.n.as<bf16>(), src, a_out, (int)E, d * (int)pm, stream)) return -1;
+  if (target_logp(m, D, a_out, (int)E, tgt, e_sc, stream)) return -1;
   return launch_gather_scores(e_sc, smap, d_scores, S * Lp, stream);
 }
 
@@ -1453,12 +1354,8 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
 static int rescoring_device(rvb_model* m, const float* d_enc_out, const int* d_elen, int B, int Tp, int N, int Lp,
                             const int* tok_l, const int* tok_r, const int* gat_l, const int* gat_r, const int* slen,
                             bool use_r, float* d_sc_l, float* d_sc_r, cudaStream_t stream) {
-  const int d = m->cfg.d_model;
-  const long long Mem = (long long)B * Tp;
-  if (m->ws_encbf.ensure((size_t)Mem * d * 2 * m->pm())) return -1;
-  bf16* encbf = m->ws_encbf.as<bf16>();
-  if (m->x3 ? launch_f32_to_pair(d_enc_out, encbf, Mem, d, stream) : launch_f32_to_bf16(d_enc_out, encbf, Mem * d, stream))
-    return -1;
+  bf16* encbf;
+  if (enc_operand(m, d_enc_out, (long long)B * Tp, &encbf, stream)) return -1;
   if (decoder_pass(m, m->dec_l, encbf, d_elen, B, Tp, N, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
   if (use_r && decoder_pass(m, m->dec_r, encbf, d_elen, B, Tp, N, Lp, tok_r, slen, gat_r, d_sc_r, stream)) return -1;
   return 0;
@@ -1706,13 +1603,8 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
     if (t.has_trie && (!use_r || t.has_rtrie)) {
       // tree-structured decoder: one row per distinct prefix of the utterance's n-best
       const int* hp_nodes = reinterpret_cast<const int*>(reinterpret_cast<const char*>(t.small.p) + t.small_bytes) + B;
-      const int d = c.d_model;
-      const long long Mem = (long long)B * Tp;
-      if (m->ws_encbf.ensure((size_t)Mem * d * 2 * m->pm())) return -1;
-      bf16* encbf = m->ws_encbf.as<bf16>();
-      if (m->x3 ? launch_f32_to_pair(t.d_enc_out, encbf, Mem, d, stream)
-                : launch_f32_to_bf16(t.d_enc_out, encbf, Mem * d, stream))
-        return -1;
+      bf16* encbf;
+      if (enc_operand(m, t.d_enc_out, (long long)B * Tp, &encbf, stream)) return -1;
       for (int dir = 0; dir < (use_r ? 2 : 1); ++dir) {
         int P = 1;
         for (int b = 0; b < B; ++b) P = hp_nodes[dir * B + b] > P ? hp_nodes[dir * B + b] : P;
@@ -1878,9 +1770,10 @@ RVB_API void rvb_model_destroy(rvb_model* m) {
   for (void* p : m->owned) cudaFree(p);
   DevBuf* bufs[] = {&m->ws_c1, &m->ws_c2, &m->ws_x, &m->ws_n, &m->ws_h, &m->ws_qkv, &m->ws_att, &m->ws_pw, &m->ws_cm,
                     &m->ws_y, &m->ws_ybf, &m->ws_pe, &m->ws_pall, &m->ws_lens, &m->ws_encbf, &m->ws_logits,
-                    &m->ws_search, &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold};
+                    &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold, &m->ws_lse, &m->ws_tree_idx,
+                    &m->ws_edge_rows, &m->ws_edge_scores, &m->ws_step_rows};
   for (DevBuf* b : bufs) b->release();
-  for (auto& b : m->ws_dec) b.release();
+  m->dec_rows.release();
   if (m->tickets) {
     for (int i = 0; i < rvb_model::kTickets; ++i) m->tickets[i].release();
     delete[] m->tickets;
@@ -1891,8 +1784,6 @@ RVB_API void rvb_model_destroy(rvb_model* m) {
   m->pin_a.release();
   m->pin_b.release();
   m->pin_c.release();
-  m->pin_d.release();
-  m->pin_e.release();
   delete m;
 }
 
