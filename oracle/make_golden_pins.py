@@ -1,7 +1,8 @@
 """Record the LIVE reference's results that pin the oracle and the synthetic-model generator
-(tests/test_oracle_vs_reference.py) -> tests/golden/pins.json + pins.npz.
+(tests/test_oracle_vs_reference.py) -> tests/golden/pins.json + pins.npz, and the encoder outputs of the convolution
+module variants the decoding pins do not cover -> tests/golden/pins_conv.json + pins_conv.npz.
 
-    python -m oracle.make_golden_pins        # needs RVB_REFERENCE_ROOT (oracle/refimport.py)
+    python -m oracle.make_golden_pins [conv]   # needs RVB_REFERENCE_ROOT (oracle/refimport.py); `conv`: only the latter
 
 Encoder outputs are stored as a fixed, seeded sample of elements plus float64 sums of the whole tensor, so that an
 exact comparison stays possible without storing the tensors.
@@ -98,5 +99,56 @@ def main():
         json.dump(meta_out, f, separators=(",", ":"))
 
 
+# Convolution-module variants at the test shape (d = 128): kernel sizes 7 and 31, causal BatchNorm, symmetric LayerNorm.
+# Each runs one zero-padded ragged batch through the full-context encoder; the symmetric ones also run the cache-based
+# chunk-by-chunk streaming pass.
+CONV_CASES = {
+    "causal_ln_k7": dict(causal=True, cnn_module_norm="layer_norm", kernel=7),
+    "sym_bn_k31": dict(causal=False, cnn_module_norm="batch_norm", kernel=31),
+    "causal_bn_k15": dict(causal=True, cnn_module_norm="batch_norm", kernel=15),
+    "sym_ln_k15": dict(causal=False, cnn_module_norm="layer_norm", kernel=15),
+}
+CONV_T, CONV_LENS, CONV_CHUNK, CONV_CAT, CONV_SEED = 403, [403, 298, 61], 16, [0.25, 0.75], 5
+
+
+def conv_case_inputs():
+    from oracle import encoder_ref
+    return encoder_ref.zero_pad(encoder_ref.features(len(CONV_LENS), CONV_T, seed=CONV_SEED), CONV_LENS)
+
+
+def conv_pins():
+    warnings.filterwarnings("ignore")
+    from oracle import refimport
+    from reverb_b200 import synth
+    wenet_ref = refimport.import_reference()
+    feats = conv_case_inputs()
+    lens = torch.tensor(CONV_LENS, dtype=torch.int32)
+    cat = torch.tensor(CONV_CAT)
+    meta_out, arrays = {"T": CONV_T, "lens": CONV_LENS, "chunk": CONV_CHUNK, "cat": CONV_CAT, "cases": {}}, {}
+    for ci, (case, kw) in enumerate(CONV_CASES.items()):
+        d = os.path.join("/tmp", f"rvb_pins_conv_{case}")
+        synth.write_model_dir(d, shape=dict(synth.TEST_SHAPE, kernel=kw["kernel"]), seed=CONV_SEED + ci,
+                              causal=kw["causal"], cnn_module_norm=kw["cnn_module_norm"])
+        m = wenet_ref.load_model(d)
+        rec = dict(kw, seed=CONV_SEED + ci)
+        with torch.no_grad():
+            enc, _ = m.model._forward_encoder(feats, lens, cat_embs=cat)
+        idx, val, s1, s2 = tensor_pin(enc, 3000 + ci)
+        arrays[f"{case}_enc_idx"], arrays[f"{case}_enc_val"] = idx, val
+        rec["enc"] = {"enc_shape": list(enc.shape), "enc_sum": s1, "enc_sumsq": s2}
+        if not kw["causal"]:
+            with torch.no_grad():
+                enc, _ = m.model.encoder.forward_chunk_by_chunk(feats[:1], CONV_CHUNK, -1, cat_embs=cat)
+            idx, val, s1, s2 = tensor_pin(enc, 4000 + ci)
+            arrays[f"{case}_stream_idx"], arrays[f"{case}_stream_val"] = idx, val
+            rec["stream"] = {"enc_shape": list(enc.shape), "enc_sum": s1, "enc_sumsq": s2}
+        meta_out["cases"][case] = rec
+    np.savez_compressed(os.path.join(GOLDEN, "pins_conv.npz"), **arrays)
+    with open(os.path.join(GOLDEN, "pins_conv.json"), "w") as f:
+        json.dump(meta_out, f, indent=1)
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] != ["conv"]:
+        main()
+    conv_pins()

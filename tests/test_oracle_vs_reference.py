@@ -1,5 +1,5 @@
 """Pins the oracle and the synthetic-model generator to the reference's own results, recorded from the live reference
-by oracle/make_golden_pins.py into tests/golden/pins.{json,npz}.  Encoder outputs are pinned by a seeded sample of
+by oracle/make_golden_pins.py into tests/golden/pins.{json,npz} and pins_conv.{json,npz}.  Encoder outputs are pinned by a seeded sample of
 elements and the float64 sums of the whole tensor; both must match exactly."""
 import json
 import os
@@ -98,6 +98,32 @@ def test_oracle_attention_mode_and_bounded_context_equal_live_reference(pins, mo
         assert len(got_c["ctc_prefix_beam_search"]) == len(want["prefix"])
         for w, c in zip(want["prefix"], got_c["ctc_prefix_beam_search"]):
             _assert_hyp(w, c, ["nbest", "nbest_scores", "nbest_times"])
+
+
+@pytest.mark.parametrize("case", ["causal_ln_k7", "sym_bn_k31", "causal_bn_k15", "sym_ln_k15"])
+def test_oracle_conv_variants_equal_live_reference(tmp_path, case):
+    """The convolution-module variants the decoding pins leave out — K = 7 and K = 31, causal BatchNorm, symmetric
+    LayerNorm — on a zero-padded ragged batch (full context) and, for the symmetric ones, the chunk-by-chunk streaming
+    pass, against the reference's encoder (oracle/make_golden_pins.py conv_pins -> tests/golden/pins_conv.*)."""
+    from oracle import make_golden_pins as mgp, model_ref, pipeline_ref
+    from reverb_b200 import synth
+    with open(os.path.join(GOLDEN, "pins_conv.json")) as f:
+        meta = json.load(f)
+    arrays = dict(np.load(os.path.join(GOLDEN, "pins_conv.npz")))
+    assert (meta["T"], meta["lens"], meta["chunk"], meta["cat"]) == (mgp.CONV_T, mgp.CONV_LENS, mgp.CONV_CHUNK, mgp.CONV_CAT)
+    rec = meta["cases"][case]
+    assert {k: rec[k] for k in ("causal", "cnn_module_norm", "kernel")} == mgp.CONV_CASES[case]
+    d = synth.write_model_dir(str(tmp_path), shape=dict(synth.TEST_SHAPE, kernel=rec["kernel"]), seed=rec["seed"],
+                              causal=rec["causal"], cnn_module_norm=rec["cnn_module_norm"])
+    orc = pipeline_ref.OracleASR(d)
+    feats = mgp.conv_case_inputs()
+    cat = torch.tensor(mgp.CONV_CAT)
+    enc, _, _ = orc.forward_encoder(feats, torch.tensor(mgp.CONV_LENS, dtype=torch.int32), cat)
+    _assert_tensor_pinned(enc, arrays, f"{case}_enc", rec["enc"])
+    assert ("stream" in rec) == (not rec["causal"])
+    if "stream" in rec:
+        enc = model_ref.encoder_forward_chunk_by_chunk(feats[:1], orc.sd, orc.cfg, cat, mgp.CONV_CHUNK)
+        _assert_tensor_pinned(enc, arrays, f"{case}_stream", rec["stream"])
 
 
 def test_oracle_resample_equals_torchaudio():
