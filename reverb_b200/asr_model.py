@@ -15,7 +15,7 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
-from .engine import Engine, check_beam_size
+from .engine import Engine, check_beam_size, nbest_lists
 from .search import (DecodeResult, attention_beam_search, greedy_results,
                      joint_decoding_results, prefix_beam_results, rescoring_pick, rescoring_pick_batch,
                      time_sync_joint_search)
@@ -201,13 +201,7 @@ class ASRModel:
         if st["ticket"] is not None:
             toks, tims, olen, scores, nhyp, l2r, r2l = self.engine.rescoring_collect(st["ticket"])
             if "ctc_prefix_beam_search" in methods:
-                per_utt = []
-                for b in range(toks.shape[0]):
-                    n = int(nhyp[b])
-                    per_utt.append(([tuple(toks[b, r, :olen[b, r, 0]].tolist()) for r in range(n)],
-                                    [float(x) for x in scores[b, :n]],
-                                    [tims[b, r, :olen[b, r, 1]].tolist() for r in range(n)]))
-                results["ctc_prefix_beam_search"] = prefix_beam_results(per_utt)
+                results["ctc_prefix_beam_search"] = prefix_beam_results(nbest_lists(toks, tims, olen, scores, nhyp))
             if "attention_rescoring" in methods:
                 results["attention_rescoring"] = rescoring_pick_batch(toks, tims, olen, scores, nhyp, l2r, r2l,
                                                                       st["ctc_weight"], st["reverse_weight"])

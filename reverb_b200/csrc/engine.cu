@@ -14,6 +14,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <map>
 #include <string>
@@ -156,6 +157,49 @@ struct DecRows {
   }
 };
 
+// The n-best of a CTC prefix beam search over B utterances, `beam` hypothesis slots each, in one device buffer and a
+// page-locked host mirror with the same layout (ints, scores 8-byte aligned):
+//   times (S rows) | encoder lens (B) | tokens (S rows) | (n_tokens, n_times) (S pairs) | nhyp (B) | pad | scores (S)
+// S = B * beam; token / time rows have stride len_cap.  Encoder lens .. nhyp is what a caller-supplied n-best uploads,
+// (n_tokens, n_times) .. scores the small region a search hands back before its tokens and times.
+struct NBest {
+  DevBuf dev;
+  HostPinned host;
+  int B = 0, beam = 0, len_cap = 0;
+  struct Arrays {
+    int *tim, *lens, *tok, *olen, *nhyp;
+    double* sc;
+  };
+  size_t S() const { return (size_t)B * beam; }
+  size_t ints() const { return (2 * S() * len_cap + 2 * S() + 2 * (size_t)B + 1) & ~(size_t)1; }  // up to scores
+  size_t bytes() const { return ints() * sizeof(int) + S() * sizeof(double); }
+  Arrays at(void* base) const {
+    Arrays a;
+    a.tim = static_cast<int*>(base);
+    a.lens = a.tim + S() * len_cap;
+    a.tok = a.lens + B;
+    a.olen = a.tok + S() * len_cap;
+    a.nhyp = a.olen + 2 * S();
+    a.sc = reinterpret_cast<double*>(static_cast<int*>(base) + ints());
+    return a;
+  }
+  Arrays d() const { return at(dev.p); }
+  Arrays h() const { return at(host.p); }
+  size_t upload_bytes() const { return (size_t)(h().nhyp + B - h().lens) * sizeof(int); }   // lens .. nhyp
+  size_t small_bytes() const { return bytes() - (size_t)(h().olen - h().tim) * sizeof(int); }  // olen .. scores
+  int ntok(size_t s) const { return (int)(s % beam) < h().nhyp[s / beam] ? h().olen[2 * s] : 0; }  // 0 when absent
+  int ensure(int B_, int beam_, int len_cap_) {
+    B = B_;
+    beam = beam_;
+    len_cap = len_cap_;
+    return (dev.ensure(bytes()) || host.ensure(bytes())) ? -1 : 0;
+  }
+  void release() {
+    dev.release();
+    host.release();
+  }
+};
+
 }  // namespace rvb
 
 using namespace rvb;
@@ -190,6 +234,8 @@ struct rvb_model {
   DevBuf ws_lse;                // output layer: OUT_LSE partials + target logits
   DevBuf ws_tree_idx, ws_edge_rows, ws_edge_scores;  // prefix-tree pass: node / edge indices, edge rows, edge scores
   DevBuf ws_step_rows;          // full log_softmax rows of the last position (decoder_step_logp)
+  DevBuf ws_search;             // prefix beam search of the tickets: they all search on s_search, one at a time
+  rvb::NBest nbest_in;          // the caller's hypotheses of rvb_attention_rescoring
   HostPinned pin_a, pin_b, pin_c;
   int pe_T = 0;
   int pall_T = 0;               // ws_pall holds linear_pos(pos_emb) for this many frames
@@ -1347,81 +1393,70 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
   return launch_gather_scores(e_sc, smap, d_scores, S * Lp, stream);
 }
 
-// Decoder passes over device-resident inputs (all int arrays on the device):
-//   tok_l / tok_r (R = S*Lp): decoder inputs [sos, w_1..w_U, eos..] and the reversed variant (asr_model.py:921-949)
-//   gat_l / gat_r (R): per-position gather targets, -1 = none (search.py:417-430);  slen (S) = U + 1;  elen (B)
-// -> d_sc_l / d_sc_r (R) log-probabilities of the targets.
-static int rescoring_device(rvb_model* m, const float* d_enc_out, const int* d_elen, int B, int Tp, int N, int Lp,
-                            const int* tok_l, const int* tok_r, const int* gat_l, const int* gat_r, const int* slen,
-                            bool use_r, float* d_sc_l, float* d_sc_r, cudaStream_t stream) {
+// The flat decoder passes over a device n-best, one row per (hypothesis, position) with Lp positions per hypothesis.
+// rescoring_inputs_kernel lays out, in idx (4 R + S ints, R = S * Lp), the decoder inputs tok_l / tok_r
+// [sos, w_1..w_U, eos..] and the reversed variant (asr_model.py:921-949), the gather targets gat_l / gat_r (-1 = none,
+// search.py:417-430) and slen = U + 1; absent hypotheses are empty.  -> d_sc_l / d_sc_r (R) log-probs of the targets.
+static int rescoring_flat(rvb_model* m, const NBest& nb, const float* d_enc_out, int Tp, int Lp, bool use_r, int* idx,
+                          float* d_sc_l, float* d_sc_r, cudaStream_t stream) {
+  const NBest::Arrays d = nb.d();
+  const size_t R = nb.S() * Lp;
+  int *tok_l = idx, *tok_r = idx + R, *gat_l = idx + 2 * R, *gat_r = idx + 3 * R, *slen = idx + 4 * R;
+  if (launch_rescoring_inputs(d.tok, nb.len_cap, d.olen, d.nhyp, nb.B, nb.beam, Lp, sos_id(m->cfg), eos_id(m->cfg), tok_l,
+                              tok_r, gat_l, gat_r, slen, stream))
+    return -1;
   bf16* encbf;
-  if (enc_operand(m, d_enc_out, (long long)B * Tp, &encbf, stream)) return -1;
-  if (decoder_pass(m, m->dec_l, encbf, d_elen, B, Tp, N, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
-  if (use_r && decoder_pass(m, m->dec_r, encbf, d_elen, B, Tp, N, Lp, tok_r, slen, gat_r, d_sc_r, stream)) return -1;
+  if (enc_operand(m, d_enc_out, (long long)nb.B * Tp, &encbf, stream)) return -1;
+  if (decoder_pass(m, m->dec_l, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
+  if (use_r && decoder_pass(m, m->dec_r, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_r, slen, gat_r, d_sc_r, stream))
+    return -1;
   return 0;
 }
 
-// position pos of the reversed pass scores token w_{U-1-pos}: store it at index j = U-1-pos
-static void unreverse_r2l(const float* src_all, const int* h_len, int len_stride, int S, int Lp, float* h_r2l) {
-  for (int s = 0; s < S; ++s) {
-    const int U = h_len[(size_t)s * len_stride] < 0 ? 0 : h_len[(size_t)s * len_stride];
-    const float* src = src_all + (size_t)s * Lp;
-    float* dst = h_r2l + (size_t)s * Lp;
-    for (int j = 0; j < Lp; ++j) dst[j] = 0.f;
-    for (int j = 0; j < U; ++j) dst[j] = src[U - 1 - j];
-    dst[U] = src[U];
-  }
+// Position j < U of the right-to-left pass scores token w_{U-1-j}: reverse [0, U) of every row in place to put the
+// scores in hypothesis order.  Position U (eos) stays; positions past it are 0 from the device (gather target -1).
+static void unreverse_r2l(const NBest& nb, int Lp, float* r2l) {
+  for (size_t s = 0; s < nb.S(); ++s) std::reverse(r2l + s * Lp, r2l + s * Lp + nb.ntok(s));
 }
 
 static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* h_enc_lens, int B, int Tp,
                                const int* h_tok, const int* h_len, int N, int max_len, const float* h_cat, int n_cat,
                                float reverse_weight, float* h_l2r, float* h_r2l, cudaStream_t stream) {
-  const rvb_model_config& c = m->cfg;
   RVB_REQUIRE(m->finalized && m->dec_l.present, "attention_rescoring: model has no decoder");
-  const int sos = sos_id(c), eos = eos_id(c);
   const int Lp = max_len + 1, S = B * N;
   const long long R = (long long)S * Lp;
   const bool use_r = reverse_weight > 0.f && m->dec_r.present && h_r2l != nullptr;
   if (fold_lang(m, h_cat, n_cat, stream)) return -1;
-  // host-side staging: decoder inputs [sos, w_1..w_U, eos..] and per-position gather targets
-  const size_t ints = (size_t)R * 4 + S + B;
-  if (m->pin_b.ensure(ints * sizeof(int)) || m->ws_misc.ensure(ints * sizeof(int) + (size_t)R * 2 * sizeof(float)))
+  // the caller's hypotheses as an n-best with every slot present: an absent row (length < 0) is an empty hypothesis
+  NBest& nb = m->nbest_in;
+  const size_t rints = (size_t)R * 4 + S;
+  if (nb.ensure(B, N, max_len) || m->ws_misc.ensure(rints * sizeof(int) + (size_t)R * 2 * sizeof(float)) ||
+      m->pin_c.ensure((size_t)R * 2 * sizeof(float)))
     return -1;
-  int* hp = m->pin_b.as<int>();
-  int* tok_l = hp;
-  int* tok_r = hp + R;
-  int* gat_l = hp + 2 * R;
-  int* gat_r = hp + 3 * R;
-  int* slen = hp + 4 * R;
-  int* elen = slen + S;
-  for (int b = 0; b < B; ++b) elen[b] = h_enc_lens[b];
+  const NBest::Arrays h = nb.h();
+  memcpy(h.lens, h_enc_lens, sizeof(int) * B);
+  memcpy(h.tok, h_tok, sizeof(int) * S * max_len);
   for (int s = 0; s < S; ++s) {
     const int U = h_len[s] < 0 ? 0 : h_len[s];
     RVB_REQUIRE(U <= max_len, "attention_rescoring: hypothesis longer than max_len");
-    const int* wv = h_tok + (size_t)s * max_len;
-    slen[s] = U + 1;
-    for (int j = 0; j < Lp; ++j) {
-      const size_t r = (size_t)s * Lp + j;
-      tok_l[r] = (j == 0) ? sos : (j <= U ? wv[j - 1] : eos);
-      tok_r[r] = (j == 0) ? sos : (j <= U ? wv[U - j] : eos);          // asr_model.py:921-949
-      gat_l[r] = (j < U) ? wv[j] : (j == U ? eos : -1);                // search.py:417-421
-      gat_r[r] = (j < U) ? wv[U - 1 - j] : (j == U ? eos : -1);        // search.py:424-430
-    }
+    h.olen[2 * s] = U;
+    h.olen[2 * s + 1] = 0;
   }
-  int* dp = m->ws_misc.as<int>();
-  RVB_CHECK_CUDA(cudaMemcpyAsync(dp, hp, ints * sizeof(int), cudaMemcpyHostToDevice, stream));
-  float* d_sc_l = reinterpret_cast<float*>(dp + ints);
+  for (int b = 0; b < B; ++b) h.nhyp[b] = N;
+  RVB_CHECK_CUDA(cudaMemcpyAsync(nb.d().lens, h.lens, nb.upload_bytes(), cudaMemcpyHostToDevice, stream));
+  int* idx = m->ws_misc.as<int>();
+  float* d_sc_l = reinterpret_cast<float*>(idx + rints);
   float* d_sc_r = d_sc_l + R;
-  if (rescoring_device(m, d_enc_out, dp + 4 * R + S, B, Tp, N, Lp, dp, dp + R, dp + 2 * R, dp + 3 * R, dp + 4 * R, use_r,
-                       d_sc_l, d_sc_r, stream))
-    return -1;
-  if (m->pin_c.ensure((size_t)R * 2 * sizeof(float))) return -1;
+  if (rescoring_flat(m, nb, d_enc_out, Tp, Lp, use_r, idx, d_sc_l, d_sc_r, stream)) return -1;
   float* hs = m->pin_c.as<float>();
   RVB_CHECK_CUDA(cudaMemcpyAsync(hs, d_sc_l, (size_t)R * (use_r ? 2 : 1) * sizeof(float), cudaMemcpyDeviceToHost,
                                  stream));
   RVB_CHECK_CUDA(cudaStreamSynchronize(stream));
   memcpy(h_l2r, hs, (size_t)R * sizeof(float));
-  if (use_r) unreverse_r2l(hs + R, h_len, 1, S, Lp, h_r2l);
+  if (use_r) {
+    unreverse_r2l(nb, Lp, hs + R);
+    memcpy(h_r2l, hs + R, (size_t)R * sizeof(float));
+  }
   return 0;
 }
 
@@ -1437,42 +1472,35 @@ static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* 
 // while the host waits for lengths or post-processes results.  Buffers that live across calls belong to the ticket.
 struct SearchTicket {
   int state = 0;      // 0 free, 1 search submitted, 2 decoder submitted
-  DevBuf out;         // lens(B) | tokens | times | out_lens (S*2) | nhyp (B) | pad | scores (S doubles)
+  NBest nb;           // rows of Tp tokens: a prefix never has more tokens than frames
   DevBuf trie;        // prefix trees of the n-best (left-to-right and reversed): node_of | node_tok | par | dep | n_nodes
-  HostPinned small;   // out_lens | nhyp | pad | scores | enc lens(B) | n_nodes (2 B)
+  HostPinned nodes;   // n_nodes of each tree (B per direction)
   int trie_cap = 0, trie_stride = 0;
   bool has_trie = false, has_rtrie = false;
   int* tr_node_of(int dir) { return trie.as<int>() + (size_t)dir * trie_ints(); }
-  size_t trie_ints() const { return (size_t)B * beam * trie_stride + (size_t)3 * B * trie_cap + B; }
+  size_t trie_ints() const { return nb.S() * trie_stride + (size_t)3 * nb.B * trie_cap + nb.B; }
   TrieView trie_view(int dir) {
     int* base = tr_node_of(dir);
     TrieView v;
     v.node_of = base;
     v.nstride = trie_stride;
-    v.node_tok = base + (size_t)B * beam * trie_stride;
-    v.node_par = const_cast<int*>(v.node_tok) + (size_t)B * trie_cap;
-    v.node_dep = const_cast<int*>(v.node_par) + (size_t)B * trie_cap;
+    v.node_tok = base + nb.S() * trie_stride;
+    v.node_par = const_cast<int*>(v.node_tok) + (size_t)nb.B * trie_cap;
+    v.node_dep = const_cast<int*>(v.node_par) + (size_t)nb.B * trie_cap;
     v.cap = trie_cap;
-    v.n_nodes = const_cast<int*>(v.node_dep) + (size_t)B * trie_cap;
+    v.n_nodes = const_cast<int*>(v.node_dep) + (size_t)nb.B * trie_cap;
     return v;
   }
   cudaEvent_t ev_search = nullptr, ev_done = nullptr;
-  int B = 0, Tp = 0, beam = 0;
-  size_t n_tok = 0, ints_al = 0, small_ints = 0, small_bytes = 0;
+  int Tp = 0;
   const float* d_enc_out = nullptr;
   int Lmax = 1;
   bool use_r = false;
   float* h_r2l = nullptr;
-  int* d_lens() { return out.as<int>(); }
-  int* d_tok() { return d_lens() + B; }
-  int* d_tim() { return d_tok() + n_tok; }
-  int* d_olen() { return d_tim() + n_tok; }
-  int* d_nhyp() { return d_olen() + (size_t)B * beam * 2; }
-  double* d_sc() { return reinterpret_cast<double*>(out.as<int>() + ints_al); }
   void release() {
-    out.release();
+    nb.release();
     trie.release();
-    small.release();
+    nodes.release();
     if (ev_search) cudaEventDestroy(ev_search);
     if (ev_done) cudaEventDestroy(ev_done);
     ev_search = ev_done = nullptr;
@@ -1486,73 +1514,67 @@ int search_side_stream(rvb_model* m, cudaStream_t* out) {
   return 0;
 }
 
+// The CTC prefix beam search into nb (rows of nb.len_cap tokens) on `stream`, with workspace ws: uploads the encoder
+// lengths through nb's host mirror, then searches, context-biased when graph != nullptr.
+static int prefix_beam_into(NBest& nb, const float* d_topk_val, const int* d_topk_idx, int k, const int* h_enc_lens,
+                            int Tp, int blank_id, DevBuf& ws, ::rvb_context_graph* graph, cudaStream_t stream) {
+  const NBest::Arrays d = nb.d(), h = nb.h();
+  if (ws.ensure(prefix_beam_workspace_bytes(nb.B, Tp, nb.beam))) return -1;
+  memcpy(h.lens, h_enc_lens, sizeof(int) * nb.B);
+  RVB_CHECK_CUDA(cudaMemcpyAsync(d.lens, h.lens, sizeof(int) * nb.B, cudaMemcpyHostToDevice, stream));
+  if (graph == nullptr)
+    return launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, d.lens, nb.B, Tp, nb.beam, blank_id, ws.p, ws.cap,
+                                  nb.len_cap, d.tok, d.tim, d.olen, d.sc, d.nhyp, stream);
+  if (launch_ctc_prefix_beam_biased(d_topk_val, d_topk_idx, k, d.lens, nb.B, Tp, nb.beam, blank_id, ws.p, ws.cap,
+                                    nb.len_cap, d.tok, d.tim, d.olen, d.sc, d.nhyp, *context_graph_view(graph), stream))
+    return -1;
+  return context_graph_note_use(graph, stream);
+}
+
 // graph != nullptr: the biased search (context biasing with that graph)
 static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val, const int* d_topk_idx, int k,
                          const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int beam, int blank_id,
-                         ::rvb_context_graph* graph, DevBuf& ws, cudaStream_t stream) {
-  const int S = B * beam, dev_len = Tp;  // a prefix never has more tokens than frames
-  t.B = B;
+                         ::rvb_context_graph* graph, cudaStream_t stream) {
   t.Tp = Tp;
-  t.beam = beam;
   t.d_enc_out = d_enc_out;
-  t.n_tok = (size_t)S * dev_len;
-  const size_t ints = B + 2 * t.n_tok + (size_t)S * 2 + B;
-  t.ints_al = (ints + 1) & ~(size_t)1;
-  const size_t out_bytes = t.ints_al * sizeof(int) + (size_t)S * sizeof(double);
-  t.small_ints = t.ints_al - (B + 2 * t.n_tok);            // out_lens | nhyp | pad
-  t.small_bytes = t.small_ints * sizeof(int) + (size_t)S * sizeof(double);
-  const size_t ws_bytes = prefix_beam_workspace_bytes(B, Tp, beam);
   // prefix trees of the n-best for the tree-structured rescoring decoder (left-to-right, and reversed when the model
   // has a right-to-left decoder): built right behind the search, their node counts travel with the lengths
   t.has_trie = rescore_trie() && m->dec_l.present && beam <= 16;
   t.has_rtrie = t.has_trie && m->dec_r.present;
-  t.trie_stride = dev_len + 1;
-  t.trie_cap = beam * dev_len + 1;
+  t.trie_stride = Tp + 1;
+  t.trie_cap = beam * Tp + 1;
   const int ndir = t.has_trie ? (t.has_rtrie ? 2 : 1) : 0;
-  if (ws.ensure(ws_bytes) || t.out.ensure(out_bytes) || t.small.ensure(t.small_bytes + sizeof(int) * B * 3) ||
+  if (t.nb.ensure(B, beam, Tp) || t.nodes.ensure(sizeof(int) * B * 2) ||
       (ndir && t.trie.ensure(t.trie_ints() * ndir * sizeof(int))))
     return -1;
   if (!t.ev_search) RVB_CHECK_CUDA(cudaEventCreateWithFlags(&t.ev_search, cudaEventDisableTiming));
   if (!t.ev_done) RVB_CHECK_CUDA(cudaEventCreateWithFlags(&t.ev_done, cudaEventDisableTiming));
-  int* hp_small = t.small.as<int>();
-  int* hp_elen = reinterpret_cast<int*>(reinterpret_cast<char*>(hp_small) + t.small_bytes);
-  memcpy(hp_elen, h_enc_lens, sizeof(int) * B);
   // The search runs on a SIDE stream: it is one CTA per utterance (64 of 132 SMs, latency-bound), so
   // in a pipelined decode the next batch's fbank / conv1 (bandwidth-bound, small CTAs) share the GPU with it instead of
   // queueing behind it.  The side stream starts after everything enqueued so far on `stream` (the CTC top-k);
   // rescoring_submit makes `stream` wait for ev_search before it touches the n-best.
-  if (m->s_search == nullptr) RVB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->s_search, cudaStreamNonBlocking));
-  if (m->ev_topk == nullptr) RVB_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_topk, cudaEventDisableTiming));
   static int side = -1;
   if (side < 0) {
     const char* e = getenv("RVB_SEARCH_STREAM");   // RVB_SEARCH_STREAM=main: keep the search on the caller's stream
     side = (e && strcmp(e, "main") == 0) ? 0 : 1;
   }
-  cudaStream_t ss = side ? m->s_search : stream;
+  cudaStream_t ss = stream;
   if (side) {
+    if (search_side_stream(m, &ss)) return -1;
+    if (m->ev_topk == nullptr) RVB_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_topk, cudaEventDisableTiming));
     RVB_CHECK_CUDA(cudaEventRecord(m->ev_topk, stream));
     RVB_CHECK_CUDA(cudaStreamWaitEvent(ss, m->ev_topk, 0));
   }
-  RVB_CHECK_CUDA(cudaMemcpyAsync(t.d_lens(), hp_elen, sizeof(int) * B, cudaMemcpyHostToDevice, ss));
-  if (graph == nullptr) {
-    if (launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, t.d_lens(), B, Tp, beam, blank_id, ws.p, ws.cap, dev_len,
-                               t.d_tok(), t.d_tim(), t.d_olen(), t.d_sc(), t.d_nhyp(), ss))
-      return -1;
-  } else {
-    if (launch_ctc_prefix_beam_biased(d_topk_val, d_topk_idx, k, t.d_lens(), B, Tp, beam, blank_id, ws.p, ws.cap,
-                                      dev_len, t.d_tok(), t.d_tim(), t.d_olen(), t.d_sc(), t.d_nhyp(),
-                                      *context_graph_view(graph), ss) ||
-        context_graph_note_use(graph, ss))
-      return -1;
-  }
-  RVB_CHECK_CUDA(cudaMemcpyAsync(hp_small, t.d_olen(), t.small_bytes, cudaMemcpyDeviceToHost, ss));
+  if (prefix_beam_into(t.nb, d_topk_val, d_topk_idx, k, h_enc_lens, Tp, blank_id, m->ws_search, graph, ss)) return -1;
+  const NBest::Arrays d = t.nb.d();
+  RVB_CHECK_CUDA(cudaMemcpyAsync(t.nb.h().olen, d.olen, t.nb.small_bytes(), cudaMemcpyDeviceToHost, ss));
   for (int dir = 0; dir < ndir; ++dir) {
     TrieView v = t.trie_view(dir);
-    if (launch_trie_build(t.d_tok(), dev_len, t.d_olen(), t.d_nhyp(), B, beam, dir, sos_id(m->cfg), const_cast<int*>(v.node_of),
+    if (launch_trie_build(d.tok, Tp, d.olen, d.nhyp, B, beam, dir, sos_id(m->cfg), const_cast<int*>(v.node_of),
                           v.nstride, const_cast<int*>(v.node_tok), const_cast<int*>(v.node_par),
                           const_cast<int*>(v.node_dep), v.cap, const_cast<int*>(v.n_nodes), ss))
       return -1;
-    RVB_CHECK_CUDA(cudaMemcpyAsync(hp_elen + B * (1 + dir), v.n_nodes, sizeof(int) * B, cudaMemcpyDeviceToHost, ss));
+    RVB_CHECK_CUDA(cudaMemcpyAsync(t.nodes.as<int>() + B * dir, v.n_nodes, sizeof(int) * B, cudaMemcpyDeviceToHost, ss));
   }
   RVB_CHECK_CUDA(cudaEventRecord(t.ev_search, ss));
   t.state = 1;
@@ -1563,13 +1585,13 @@ static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val,
 static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, int n_cat, float reverse_weight, int cap,
                             int run_decoder, int* h_tokens, int* h_times, float* h_l2r, float* h_r2l, int* out_max_len,
                             cudaStream_t stream) {
-  const rvb_model_config& c = m->cfg;
   RVB_REQUIRE(t.state == 1, "rescoring_submit: ticket has no submitted search");
-  const int B = t.B, N = t.beam, S = B * N, dev_len = t.Tp, Tp = t.Tp;
+  const int B = t.nb.B, N = t.nb.beam, S = B * N, Tp = t.Tp;
   RVB_CHECK_CUDA(cudaEventSynchronize(t.ev_search));
   RVB_CHECK_CUDA(cudaStreamWaitEvent(stream, t.ev_search, 0));   // the n-best was produced on the side stream
-  const int* ol = t.small.as<int>();
-  const int* nh = ol + (size_t)S * 2;
+  const NBest::Arrays d = t.nb.d();
+  const int* ol = t.nb.h().olen;
+  const int* nh = t.nb.h().nhyp;
   int Lmax = 1;
   for (int b = 0; b < B; ++b)
     for (int i = 0; i < N; ++i) {
@@ -1579,13 +1601,13 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
         Lmax = ol[2 * s + 1] > Lmax ? ol[2 * s + 1] : Lmax;
       }
     }
-  RVB_REQUIRE(Lmax <= cap && Lmax <= dev_len, "beam_search_rescoring: hypothesis of %d tokens exceeds capacity %d", Lmax, cap);
+  RVB_REQUIRE(Lmax <= cap && Lmax <= Tp, "beam_search_rescoring: hypothesis of %d tokens exceeds capacity %d", Lmax, cap);
   *out_max_len = Lmax;
   t.Lmax = Lmax;
   // n-best tokens / times -> caller's host buffers (compact rows of Lmax), overlapping the decoder on the copy engine
-  RVB_CHECK_CUDA(cudaMemcpy2DAsync(h_tokens, (size_t)Lmax * sizeof(int), t.d_tok(), (size_t)dev_len * sizeof(int),
+  RVB_CHECK_CUDA(cudaMemcpy2DAsync(h_tokens, (size_t)Lmax * sizeof(int), d.tok, (size_t)Tp * sizeof(int),
                                    (size_t)Lmax * sizeof(int), (size_t)S, cudaMemcpyDeviceToHost, stream));
-  RVB_CHECK_CUDA(cudaMemcpy2DAsync(h_times, (size_t)Lmax * sizeof(int), t.d_tim(), (size_t)dev_len * sizeof(int),
+  RVB_CHECK_CUDA(cudaMemcpy2DAsync(h_times, (size_t)Lmax * sizeof(int), d.tim, (size_t)Tp * sizeof(int),
                                    (size_t)Lmax * sizeof(int), (size_t)S, cudaMemcpyDeviceToHost, stream));
   t.use_r = false;
   t.h_r2l = nullptr;
@@ -1602,24 +1624,19 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
     float* d_sc_r = d_sc_l + R;
     if (t.has_trie && (!use_r || t.has_rtrie)) {
       // tree-structured decoder: one row per distinct prefix of the utterance's n-best
-      const int* hp_nodes = reinterpret_cast<const int*>(reinterpret_cast<const char*>(t.small.p) + t.small_bytes) + B;
+      const int* hp_nodes = t.nodes.as<int>();
       bf16* encbf;
       if (enc_operand(m, t.d_enc_out, (long long)B * Tp, &encbf, stream)) return -1;
       for (int dir = 0; dir < (use_r ? 2 : 1); ++dir) {
         int P = 1;
         for (int b = 0; b < B; ++b) P = hp_nodes[dir * B + b] > P ? hp_nodes[dir * B + b] : P;
         P = (P + 7) & ~7;
-        if (decoder_pass_trie(m, dir ? m->dec_r : m->dec_l, encbf, t.d_lens(), B, Tp, N, Lp, P, t.trie_view(dir),
-                              t.d_olen(), t.d_nhyp(), dir ? d_sc_r : d_sc_l, stream))
+        if (decoder_pass_trie(m, dir ? m->dec_r : m->dec_l, encbf, d.lens, B, Tp, N, Lp, P, t.trie_view(dir), d.olen,
+                              d.nhyp, dir ? d_sc_r : d_sc_l, stream))
           return -1;
       }
-    } else {
-      if (launch_rescoring_inputs(t.d_tok(), dev_len, t.d_olen(), t.d_nhyp(), B, N, Lp, sos_id(c), eos_id(c), dp, dp + R,
-                                  dp + 2 * R, dp + 3 * R, dp + 4 * R, stream))
-        return -1;
-      if (rescoring_device(m, t.d_enc_out, t.d_lens(), B, Tp, N, Lp, dp, dp + R, dp + 2 * R, dp + 3 * R, dp + 4 * R, use_r,
-                           d_sc_l, d_sc_r, stream))
-        return -1;
+    } else if (rescoring_flat(m, t.nb, t.d_enc_out, Tp, Lp, use_r, dp, d_sc_l, d_sc_r, stream)) {
+      return -1;
     }
     RVB_CHECK_CUDA(cudaMemcpyAsync(h_l2r, d_sc_l, (size_t)R * sizeof(float), cudaMemcpyDeviceToHost, stream));
     if (use_r) {
@@ -1636,27 +1653,11 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
 static int rescoring_collect(SearchTicket& t, int* h_lens, double* h_scores, int* h_nhyp) {
   RVB_REQUIRE(t.state == 2, "rescoring_collect: ticket has no submitted decoder pass");
   RVB_CHECK_CUDA(cudaEventSynchronize(t.ev_done));
-  const int B = t.B, N = t.beam, S = B * N, Lp = t.Lmax + 1;
-  const int* ol = t.small.as<int>();
-  const int* nh = ol + (size_t)S * 2;
-  memcpy(h_lens, ol, (size_t)S * 2 * sizeof(int));
-  memcpy(h_nhyp, nh, sizeof(int) * B);
-  memcpy(h_scores, reinterpret_cast<const char*>(ol) + t.small_ints * sizeof(int), (size_t)S * sizeof(double));
-  if (t.use_r) {
-    // position pos of the reversed pass scores token w_{U-1-pos}: re-index to hypothesis order in place; absent
-    // hypotheses (i >= nhyp) were scored as empty (length 0)
-    for (int b = 0; b < B; ++b)
-      for (int i = 0; i < N; ++i) {
-        const size_t s = (size_t)b * N + i;
-        const int U = (i < nh[b]) ? ol[2 * s] : 0;
-        float* row = t.h_r2l + s * Lp;
-        for (int j = 0; j < U / 2; ++j) {
-          const float tmp = row[j];
-          row[j] = row[U - 1 - j];
-          row[U - 1 - j] = tmp;
-        }
-      }
-  }
+  const NBest::Arrays h = t.nb.h();
+  memcpy(h_lens, h.olen, t.nb.S() * 2 * sizeof(int));
+  memcpy(h_nhyp, h.nhyp, sizeof(int) * t.nb.B);
+  memcpy(h_scores, h.sc, t.nb.S() * sizeof(double));
+  if (t.use_r) unreverse_r2l(t.nb, t.Lmax + 1, t.h_r2l);
   t.state = 0;
   return 0;
 }
@@ -1771,9 +1772,10 @@ RVB_API void rvb_model_destroy(rvb_model* m) {
   DevBuf* bufs[] = {&m->ws_c1, &m->ws_c2, &m->ws_x, &m->ws_n, &m->ws_h, &m->ws_qkv, &m->ws_att, &m->ws_pw, &m->ws_cm,
                     &m->ws_y, &m->ws_ybf, &m->ws_pe, &m->ws_pall, &m->ws_lens, &m->ws_encbf, &m->ws_logits,
                     &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold, &m->ws_lse, &m->ws_tree_idx,
-                    &m->ws_edge_rows, &m->ws_edge_scores, &m->ws_step_rows};
+                    &m->ws_edge_rows, &m->ws_edge_scores, &m->ws_step_rows, &m->ws_search};
   for (DevBuf* b : bufs) b->release();
   m->dec_rows.release();
+  m->nbest_in.release();
   if (m->tickets) {
     for (int i = 0; i < rvb_model::kTickets; ++i) m->tickets[i].release();
     delete[] m->tickets;
@@ -1862,9 +1864,11 @@ RVB_API int rvb_logp_topk(const float* d_logp, int rows, int V, int k, float* d_
   return rvb::launch_logsoftmax_topk(d_logp, V, rows, V, k, d_topk_val, d_topk_idx, nullptr, 0, (cudaStream_t)stream);
 }
 
-// per host thread: two decoding lanes (threads) may run the searches concurrently
+// per host thread: two decoding lanes (threads) may run the searches concurrently.  The model-less synchronous
+// searches only: the prefix beam search (workspace, n-best) and the greedy search (outputs, host copy).
 static thread_local rvb::DevBuf g_search_ws, g_search_out;
 static thread_local rvb::HostPinned g_search_pin;
+static thread_local rvb::NBest g_search_nb;
 
 RVB_API int rvb_ctc_greedy_search(const int* d_topk_idx, int k, const int* h_enc_lens, int B, int Tp, int blank_id,
                           int* h_tokens, int* h_lens, void* stream_) {
@@ -1892,41 +1896,21 @@ static int prefix_beam_search(const float* d_topk_val, const int* d_topk_idx, in
   RVB_REQUIRE(d_topk_val && d_topk_idx && h_enc_lens && h_tokens && h_times && h_lens && h_scores && h_nhyp && B > 0 &&
                   Tp > 0 && max_len > 0,
               "rvb_ctc_prefix_beam_search: bad arguments");
-  const size_t ws_bytes = rvb::prefix_beam_workspace_bytes(B, Tp, beam);
-  const size_t n_tok = (size_t)B * beam * max_len;
-  // device outputs: lens(B) | tokens | times | out_lens (B*beam*2) | nhyp (B) | scores (B*beam doubles, 8-aligned)
-  const size_t ints = B + 2 * n_tok + (size_t)B * beam * 2 + B;
-  const size_t ints_al = (ints + 1) & ~(size_t)1;
-  const size_t out_bytes = ints_al * sizeof(int) + (size_t)B * beam * sizeof(double);
-  if (g_search_ws.ensure(ws_bytes) || g_search_out.ensure(out_bytes) || g_search_pin.ensure(out_bytes)) return -1;
-  int* d_lens = g_search_out.as<int>();
-  int* d_tok = d_lens + B;
-  int* d_tim = d_tok + n_tok;
-  int* d_olen = d_tim + n_tok;
-  int* d_nhyp = d_olen + (size_t)B * beam * 2;
-  double* d_sc = reinterpret_cast<double*>(g_search_out.as<int>() + ints_al);
-  int* hp = g_search_pin.as<int>();
-  memcpy(hp, h_enc_lens, sizeof(int) * B);
-  RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, hp, sizeof(int) * B, cudaMemcpyHostToDevice, stream));
-  RVB_CHECK_CUDA(cudaMemsetAsync(d_tok, 0, (ints - B) * sizeof(int), stream));
-  if (graph == nullptr) {
-    if (rvb::launch_ctc_prefix_beam(d_topk_val, d_topk_idx, k, d_lens, B, Tp, beam, blank_id, g_search_ws.p,
-                                    g_search_ws.cap, max_len, d_tok, d_tim, d_olen, d_sc, d_nhyp, stream))
-      return -1;
-  } else {
-    if (rvb::launch_ctc_prefix_beam_biased(d_topk_val, d_topk_idx, k, d_lens, B, Tp, beam, blank_id, g_search_ws.p,
-                                           g_search_ws.cap, max_len, d_tok, d_tim, d_olen, d_sc, d_nhyp,
-                                           *rvb::context_graph_view(graph), stream) ||
-        rvb::context_graph_note_use(graph, stream))
-      return -1;
-  }
-  RVB_CHECK_CUDA(cudaMemcpyAsync(hp, g_search_out.p, out_bytes, cudaMemcpyDeviceToHost, stream));
+  rvb::NBest& nb = g_search_nb;
+  if (nb.ensure(B, beam, max_len)) return -1;
+  const rvb::NBest::Arrays d = nb.d(), h = nb.h();
+  // zero every output (token / time rows read 0 past a hypothesis' end); the lens slot in between is uploaded after
+  RVB_CHECK_CUDA(cudaMemsetAsync(d.tim, 0, (size_t)(d.nhyp + B - d.tim) * sizeof(int), stream));
+  if (rvb::prefix_beam_into(nb, d_topk_val, d_topk_idx, k, h_enc_lens, Tp, blank_id, g_search_ws, graph, stream))
+    return -1;
+  RVB_CHECK_CUDA(cudaMemcpyAsync(nb.host.p, nb.dev.p, nb.bytes(), cudaMemcpyDeviceToHost, stream));
   RVB_CHECK_CUDA(cudaStreamSynchronize(stream));
-  memcpy(h_tokens, hp + B, n_tok * sizeof(int));
-  memcpy(h_times, hp + B + n_tok, n_tok * sizeof(int));
-  memcpy(h_lens, hp + B + 2 * n_tok, (size_t)B * beam * 2 * sizeof(int));
-  memcpy(h_nhyp, hp + B + 2 * n_tok + (size_t)B * beam * 2, sizeof(int) * B);
-  memcpy(h_scores, hp + ints_al, (size_t)B * beam * sizeof(double));
+  const size_t n_tok = nb.S() * max_len;
+  memcpy(h_tokens, h.tok, n_tok * sizeof(int));
+  memcpy(h_times, h.tim, n_tok * sizeof(int));
+  memcpy(h_lens, h.olen, nb.S() * 2 * sizeof(int));
+  memcpy(h_nhyp, h.nhyp, sizeof(int) * B);
+  memcpy(h_scores, h.sc, nb.S() * sizeof(double));
   for (size_t i = 0; i < (size_t)B * beam; ++i) {
     RVB_REQUIRE(h_lens[2 * i] <= max_len && h_lens[2 * i + 1] <= max_len,
                 "rvb_ctc_prefix_beam_search: hypothesis of %d tokens exceeds max_len=%d", h_lens[2 * i], max_len);
@@ -1970,7 +1954,7 @@ static int search_submit_any(rvb_model* m, const float* d_topk_val, const int* d
   RVB_REQUIRE(id >= 0, "rvb_search_submit: all %d tickets of this plan are in flight (collect one first)",
               rvb_model::kTickets);
   if (rvb::search_submit(m, m->tickets[id], d_topk_val, d_topk_idx, k, d_enc_out, h_enc_lens, B, Tp, beam, blank_id,
-                         graph, g_search_ws, (cudaStream_t)stream)) {
+                         graph, (cudaStream_t)stream)) {
     m->tickets[id].state = 0;
     return -1;
   }

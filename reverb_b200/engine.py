@@ -34,6 +34,18 @@ def _np_ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def nbest_lists(toks, tims, olen, scores, nhyp) -> List[Tuple[List[tuple], List[float], List[List[int]]]]:
+    """An n-best as arrays (Engine.prefix_beam_search_raw, Engine.rescoring_collect) -> per utterance
+    (nbest tokens [tuple], nbest scores [float], nbest times [list])."""
+    out = []
+    for b in range(toks.shape[0]):
+        n = int(nhyp[b])
+        out.append(([tuple(toks[b, r, :olen[b, r, 0]].tolist()) for r in range(n)],
+                    [float(s) for s in scores[b, :n]],
+                    [tims[b, r, :olen[b, r, 1]].tolist() for r in range(n)]))
+    return out
+
+
 PRECISIONS = {"bf16": 0, "fp32": 1, "bf16x3": 1}
 
 
@@ -340,32 +352,17 @@ class Engine:
         scores = np.zeros((B, beam), dtype=np.float64)
         nhyp = np.zeros(B, dtype=np.int32)
         dg = None if context is None else self.device_context_graph(context, blank_id)
+        fn, graph = ((self.lib.rvb_ctc_prefix_beam_search, ()) if dg is None else
+                     (self.lib.rvb_ctc_prefix_beam_search_biased, (dg._h,)))
         with torch.cuda.device(self.device):
-            if dg is None:
-                check(self.lib.rvb_ctc_prefix_beam_search(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp, beam,
-                                                          int(blank_id), max_len, _np_ptr(toks), _np_ptr(tims),
-                                                          _np_ptr(olen), _np_ptr(scores), _np_ptr(nhyp), self._stream()),
-                      "rvb_ctc_prefix_beam_search")
-            else:
-                check(self.lib.rvb_ctc_prefix_beam_search_biased(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp,
-                                                                 beam, int(blank_id), max_len, _np_ptr(toks),
-                                                                 _np_ptr(tims), _np_ptr(olen), _np_ptr(scores),
-                                                                 _np_ptr(nhyp), dg._h, self._stream()),
-                      "rvb_ctc_prefix_beam_search_biased")
+            check(fn(_ptr(topk_val), _ptr(topk_idx), k, _np_ptr(lens), B, Tp, beam, int(blank_id), max_len, _np_ptr(toks),
+                     _np_ptr(tims), _np_ptr(olen), _np_ptr(scores), _np_ptr(nhyp), *graph, self._stream()), fn.__name__)
         return toks, tims, olen, scores, nhyp
 
     def prefix_beam_search(self, topk_val: torch.Tensor, topk_idx: torch.Tensor, enc_lens, beam: int,
                            blank_id: int = 0, context=None):
         """-> per utterance (nbest tokens [tuple], nbest scores [float], nbest times [list])."""
-        toks, tims, olen, scores, nhyp = self.prefix_beam_search_raw(topk_val, topk_idx, enc_lens, beam, blank_id,
-                                                                     context)
-        out = []
-        for b in range(toks.shape[0]):
-            n = int(nhyp[b])
-            nbest = [tuple(toks[b, r, :olen[b, r, 0]].tolist()) for r in range(n)]
-            times = [tims[b, r, :olen[b, r, 1]].tolist() for r in range(n)]
-            out.append((nbest, [float(s) for s in scores[b, :n]], times))
-        return out
+        return nbest_lists(*self.prefix_beam_search_raw(topk_val, topk_idx, enc_lens, beam, blank_id, context))
 
     # ---- prefix beam search (+ attention rescoring) as three stages around a native ticket, so that one host thread
     # can software-pipeline consecutive batches (asr_model.ASRModel.decode_stream): see include/rvb_b200.h
@@ -377,13 +374,10 @@ class Engine:
         lens = np.ascontiguousarray(np.asarray(enc_lens, dtype=np.int32))
         enc_out = enc_out.contiguous()
         dg = None if context is None else self.device_context_graph(context, blank_id)
+        fn, graph = (self.lib.rvb_search_submit, ()) if dg is None else (self.lib.rvb_search_submit_biased, (dg._h,))
         with torch.cuda.device(self.device):
-            if dg is None:
-                tid = self.lib.rvb_search_submit(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out), _np_ptr(lens),
-                                                 B, Tp, beam, int(blank_id), self._stream())
-            else:
-                tid = self.lib.rvb_search_submit_biased(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out),
-                                                        _np_ptr(lens), B, Tp, beam, int(blank_id), dg._h, self._stream())
+            tid = fn(self._h, _ptr(topk_val), _ptr(topk_idx), k, _ptr(enc_out), _np_ptr(lens), B, Tp, beam, int(blank_id),
+                     *graph, self._stream())
         if tid < 0:
             raise RuntimeError("rvb_search_submit failed: " + _lib.last_error())
         return {"id": tid, "B": B, "Tp": Tp, "beam": beam, "cap": max(int(lens.max()) if B else 1, 1),
