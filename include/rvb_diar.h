@@ -83,6 +83,18 @@ RVB_API int rvb_emb_num_frames(const rvb_emb_model* m, int num_samples);
 RVB_API int rvb_emb_forward(rvb_emb_model* m, const float* d_wave, int B, int num_samples, const float* d_weights, int S,
                             int Tw, float* d_emb, float* d_fbank, void* stream);
 
+/* ---- centroid-linkage agglomerative clustering ---------------------------------------------------------------------
+ * scipy.cluster.hierarchy.linkage(emb, method="centroid", metric="euclidean") on the device: the same Z, bit for bit,
+ * whenever no two candidate merge heights tie.  Ties go to the smallest height, then the smallest slot pair (a, b)
+ * (scipy's heap may choose differently there).  Z rows come in merge order, unsorted (centroid linkage has inversions).
+ * The condensed distance matrix, n (n - 1) / 2 doubles, lives in the caller's workspace; nothing else bounds n. */
+/* bytes of workspace for n embeddings; -1 when n < 2 or n is beyond any device */
+RVB_API long long rvb_centroid_linkage_workspace_bytes(int n);
+/* d_emb (n, dim) fp64, unit-normalised; d_Z (n - 1, 4) fp64 (cluster, cluster, height, size).  d_dist (optional,
+ * n (n - 1) / 2 fp64): the pairwise distances in scipy's pdist order, before any merge. */
+RVB_API int rvb_centroid_linkage(const double* d_emb, int n, int dim, double* d_Z, double* d_dist, void* d_workspace,
+                                 long long workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -116,6 +116,8 @@ SIGNATURES = {
     "rvb_emb_destroy": (None, [_vp]),
     "rvb_emb_num_frames": (_i, [_vp, _i]),
     "rvb_emb_forward": (_i, [_vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "rvb_centroid_linkage_workspace_bytes": (_ll, [_i]),
+    "rvb_centroid_linkage": (_i, [_vp, _i, _i, _vp, _vp, _vp, _ll, _vp]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -9,9 +9,9 @@ i.e. `pyannote.audio.pipelines.SpeakerDiarization.apply` (pyannote.audio==3.3.1,
 ** parity unpinned **: pyannote's source is absent offline; this module restates the PUBLISHED algorithm of that
 pipeline (3.1 defaults: 10 s windows every 1 s, powerset segmentation, overlap-excluded masked embeddings,
 centroid-linkage agglomerative clustering at threshold 0.7046 with min_cluster_size 12, count-constrained
-reconstruction) step by step, naming the upstream function each step follows.  The two networks run on the GPU; the
-glue (aggregation over windows, clustering of a few hundred 256-d vectors, run-length encoding) is host numpy/scipy,
-as it is CPU numpy/scipy upstream.
+reconstruction) step by step, naming the upstream function each step follows.  The two networks and the centroid
+linkage (thousands of 256-d vectors for a long call; csrc/diar_cluster.cu) run on the GPU; the rest of the glue
+(aggregation over windows, cutting the dendrogram, run-length encoding) is host numpy/scipy, as it is upstream.
 """
 from __future__ import annotations
 
@@ -97,11 +97,42 @@ def condensed_euclidean(emb: np.ndarray, device: Optional[str] = None) -> np.nda
     return d[iu[0], iu[1]].cpu().numpy()
 
 
+def centroid_linkage(emb: np.ndarray, device, return_distances: bool = False):
+    """scipy `linkage(emb, method="centroid", metric="euclidean")` on a CUDA device (csrc/diar_cluster.cu): the same Z
+    bit for bit unless two candidate merge heights tie (then the smallest pair (a, b) merges first).  The n (n - 1) / 2
+    pairwise distances live in device memory for the call.  `return_distances` also returns them (scipy's pdist)."""
+    from .. import _lib
+    lib = _lib.load()
+    x = np.ascontiguousarray(emb, dtype=np.float64)
+    n, dim = x.shape
+    if not np.isfinite(x).all():
+        raise ValueError("The condensed distance matrix must contain only finite values.")   # scipy's check
+    need = int(lib.rvb_centroid_linkage_workspace_bytes(n))
+    if need < 0:
+        raise ValueError(f"centroid linkage needs 2 or more embeddings and a workspace that fits a counter, got n = {n}")
+    device = torch.device(device)
+    try:
+        ws = torch.empty(need, dtype=torch.uint8, device=device)
+    except torch.OutOfMemoryError as e:
+        raise RuntimeError(f"centroid linkage of {n} embeddings needs {need / 2**30:.2f} GiB of device memory for the "
+                           f"pairwise distances, more than {device} has free") from e
+    xd = torch.from_numpy(x).to(device)
+    Z = torch.empty((n - 1, 4), dtype=torch.float64, device=device)
+    dist = torch.empty(n * (n - 1) // 2, dtype=torch.float64, device=device) if return_distances else None
+    with torch.cuda.device(device):
+        _lib.check(lib.rvb_centroid_linkage(xd.data_ptr(), n, dim, Z.data_ptr(),
+                                            dist.data_ptr() if dist is not None else None, ws.data_ptr(), need,
+                                            torch.cuda.current_stream(device).cuda_stream), "rvb_centroid_linkage")
+        Z = Z.cpu().numpy()
+    return (Z, dist.cpu().numpy()) if return_distances else Z
+
+
 def agglomerative_clustering(embeddings: np.ndarray, threshold: float, min_cluster_size: int,
                              device: Optional[str] = None) -> np.ndarray:
     """`AgglomerativeClustering.cluster` (method "centroid", metric "cosine"): unit-normalise, centroid linkage on
     Euclidean distances, cut at `threshold`, then merge every small cluster (< min_cluster_size members) into the large
-    cluster with the nearest centroid (cosine) and renumber from 0."""
+    cluster with the nearest centroid (cosine) and renumber from 0.  On a CUDA `device` the linkage runs on it
+    (centroid_linkage); the dendrogram is scipy's."""
     from scipy.cluster.hierarchy import fcluster, linkage
     from scipy.spatial.distance import cdist
     n = embeddings.shape[0]
@@ -110,7 +141,9 @@ def agglomerative_clustering(embeddings: np.ndarray, threshold: float, min_clust
         return np.zeros((1,), np.int64)
     with np.errstate(divide="ignore", invalid="ignore"):
         emb = embeddings / np.linalg.norm(embeddings, axis=-1, keepdims=True)
-    if device is not None and n > 256:
+    if device is not None and torch.device(device).type == "cuda":
+        dendrogram = centroid_linkage(emb, device)
+    elif device is not None and n > 256:
         dendrogram = linkage(condensed_euclidean(emb, device), method="centroid")
     else:
         dendrogram = linkage(emb, method="centroid", metric="euclidean")

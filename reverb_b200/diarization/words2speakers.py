@@ -18,11 +18,12 @@ give.  Everything else is deterministic and identical.
 from __future__ import annotations
 
 import csv
+import io
 from typing import Iterable, Iterator, List, Sequence, TextIO, Tuple
 
 import numpy as np
 
-from .rttm import Turn, load_rttm
+from .rttm import Turn, load_rttm, write_rttm
 
 
 def read_ctm(ctm_path: str) -> Iterator[List[str]]:
@@ -97,6 +98,25 @@ def write_stm(diarization_rttm: str, ctm_transcription: str, output_stm_transcri
     with open(output_stm_transcription, "w") as f:
         for ln in lines:
             f.write(ln + "\n")
+
+
+def rttm_text(uri: str, turns: Iterable[Turn]) -> str:
+    """What `diarization.infer` writes to `<uri>.rttm` for these turns."""
+    f = io.StringIO()
+    write_rttm(f, uri, turns)
+    return f.getvalue()
+
+
+def stm_text(uri: str, rttm: str, ctm: str) -> str:
+    """`write_stm` on an RTTM of `uri` and a CTM held in memory -> the text it writes.  Both go through the same readers
+    as the files (the RTTM through load_rttm, the CTM through the csv reader with universal newlines), so the STM is
+    byte-identical to the one the file chain writes.  An RTTM without turns (where write_stm finds no uri) gives every
+    word the speaker ""."""
+    parsed = load_rttm(io.StringIO(rttm))
+    assert list(parsed.keys()) in ([], [uri]), list(parsed.keys())
+    turns = parsed.get(uri, [])
+    rows = csv.reader(io.StringIO(ctm, newline=None), delimiter=" ")
+    return "".join(ln + "\n" for ln in assign_words_to_speakers(rows, turns, uri))
 
 
 def main(argv=None) -> None:

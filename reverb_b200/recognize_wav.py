@@ -3,6 +3,8 @@ asr/wenet/bin/recognize_wav.py (flags :33-145, `<result_dir>/<mode>/<audio stem>
 
     python -m reverb_b200.recognize_wav --model <dir> --audio_file a.wav --result_dir out
     python -m reverb_b200.recognize_wav --model <dir> --audio_file calls/*.wav --result_dir out   # batched together
+    python -m reverb_b200.recognize_wav --model <dir> --audio_file call.wav --result_dir out --diarization_model dia
+        # + out/<mode>/call.stm (a speaker on every word) and out/rttm/call.rttm
 """
 from __future__ import annotations
 
@@ -55,6 +57,11 @@ def get_args(argv=None):
                         "ctc_prefix_beam_search and attention_rescoring")
     p.add_argument("--context_graph_score", type=float, default=6.0,
                    help="Bonus per matched token of a --context_list_path phrase")
+    p.add_argument("--diarization_model", default=None,
+                   help="Directory with segmentation.pt and embedding.pt (as diarization.infer --pipeline-model): also "
+                        "write <result_dir>/<mode>/<stem>.stm and <result_dir>/rttm/<stem>.rttm")
+    p.add_argument("--diarization_synthetic", action="store_true",
+                   help="Like --diarization_model, with the seeded synthetic diarization weights")
     p.add_argument("--log_level", choices=["DEBUG", "INFO", "WARNING", "ERROR", "CRITICAL"], default="INFO")
     return p.parse_args(argv)
 
@@ -89,6 +96,11 @@ def main(argv=None):
     for mode in args.modes:
         out_dirs.append(Path(args.result_dir) / mode)
         os.makedirs(out_dirs[-1], exist_ok=True)
+    diarization = None
+    if args.diarization_model or args.diarization_synthetic:
+        from .diarization.infer import load_pipeline
+        diarization = load_pipeline(args.diarization_model, synthetic=args.diarization_synthetic)
+        os.makedirs(Path(args.result_dir) / "rttm", exist_ok=True)
     graph = asr.context_graph(args.context_list_path, args.context_graph_score) if args.context_list_path else None
     results = asr.transcribe_files(
         args.audio_file, modes=args.modes, format="ctm", verbatimicity=args.verbatimicity,
@@ -97,10 +109,19 @@ def main(argv=None):
         ctc_weight=args.ctc_weight, simulate_streaming=args.simulate_streaming, reverse_weight=args.reverse_weight,
         blank_penalty=args.blank_penalty, length_penalty=args.length_penalty,
         timings_adjustment=args.timings_adjustment, context_graph=graph)
-    for name, (_, outputs) in zip(names, results):
+    for name, (path, outputs) in zip(names, results):
         for out_dir, text in zip(out_dirs, outputs):
             with (out_dir / name).open(mode="w") as fp:
                 fp.write(text)
+        if diarization is not None:
+            from .reverb import speaker_outputs
+            rttm, stms = speaker_outputs(diarization, path, outputs)
+            stem = Path(name).stem
+            with (Path(args.result_dir) / "rttm" / f"{stem}.rttm").open(mode="w") as fp:
+                fp.write(rttm)
+            for out_dir, text in zip(out_dirs, stms):
+                with (out_dir / f"{stem}.stm").open(mode="w") as fp:
+                    fp.write(text)
 
 
 if __name__ == "__main__":

@@ -184,15 +184,19 @@ class ReverbASR:
                          chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
                          decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                          simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
-                         length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None) -> list[str]:
+                         length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None,
+                         diarization=None) -> list[str]:
         """context_graph: phrases to boost in ctc_prefix_beam_search / attention_rescoring (ReverbASR.context_graph, or
-        either ContextGraph form); the other modes ignore it, like the reference's decode()."""
+        either ContextGraph form); the other modes ignore it, like the reference's decode().
+        format="stm" with `diarization` (a SpeakerDiarization, e.g. diarization.infer.load_pipeline()): a speaker on
+        every word, see transcribe_files."""
         for _, outputs in self.transcribe_files(
                 [audio_file], modes, format=format, verbatimicity=verbatimicity, chunk_size=chunk_size,
                 batch_size=batch_size, beam_size=beam_size, decoding_chunk_size=decoding_chunk_size,
                 num_decoding_left_chunks=num_decoding_left_chunks, ctc_weight=ctc_weight,
                 simulate_streaming=simulate_streaming, reverse_weight=reverse_weight, blank_penalty=blank_penalty,
-                length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph):
+                length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph,
+                diarization=diarization):
             pass
         return outputs
 
@@ -201,7 +205,7 @@ class ReverbASR:
                          decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                          simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
                          length_penalty: float = 0.0, timings_adjustment: float = 230,
-                         context_graph=None) -> Iterator[Tuple[str, List[str]]]:
+                         context_graph=None, diarization=None) -> Iterator[Tuple[str, List[str]]]:
         """Transcribes many recordings with one set of decode settings -> (audio_file, [output per mode]) in input
         order, each as soon as it and every earlier recording are decoded.  Every output is the one
         `transcribe_modes(audio_file, ...)` gives on its own.
@@ -210,7 +214,16 @@ class ReverbASR:
         DESIGN.md §4f).  Files are read and parsed on a background thread, one window of recordings ahead; upload,
         resampling, fbank and decoding run on the caller's thread and current stream (or the lanes of `set_lanes`).
         A file that cannot be read, or has under 400 samples, raises the error `transcribe` raises, naming the file,
-        after the outputs of every earlier file; no batch holding its chunks is decoded."""
+        after the outputs of every earlier file; no batch holding its chunks is decoded.
+
+        format="stm" needs `diarization` (a SpeakerDiarization, e.g. diarization.infer.load_pipeline()) and only it
+        takes one.  Each output is then the STM that the file chain diarization.infer (RTTM, uri = the file's stem) ->
+        recognize_wav (CTM) -> words2speakers writes, byte for byte.  Diarization runs once per recording, on all of its
+        channels downmixed (infer.read_audio; the ASR reads channel 0), on the caller's thread and current stream as
+        the recording is yielded."""
+        if (format == "stm") != (diarization is not None):   # fail before any audio is read
+            raise ValueError('format="stm" and diarization= go together: a speaker-attributed transcript needs a '
+                             'SpeakerDiarization, and only format="stm" uses one')
         check_beam_size(beam_size)        # fail before any audio is read / decoded (limit: engine.MAX_BEAM_SIZE)
         if context_graph is not None:     # upload (and check) the graph once, before any audio is read
             context_graph = self.engine.device_context_graph(context_graph, self.blank_id)
@@ -270,10 +283,13 @@ class ReverbASR:
                     rec.left -= 1
                 while waiting and waiting[0].left == 0:
                     rec = waiting.popleft()
-                    yield rec.path, [get_output(format, self.tokenizer, Path(rec.path).name,
-                                                [rec.hyps[mode][c] for c in range(rec.chunks)],
-                                                timings_adjustment, chunk_size, self.input_frame_length,
-                                                self.output_frame_length) for mode in modes]
+                    outputs = [get_output("ctm" if diarization is not None else format, self.tokenizer,
+                                          Path(rec.path).name, [rec.hyps[mode][c] for c in range(rec.chunks)],
+                                          timings_adjustment, chunk_size, self.input_frame_length,
+                                          self.output_frame_length) for mode in modes]
+                    if diarization is not None:
+                        outputs = speaker_outputs(diarization, rec.path, outputs)[1]
+                    yield rec.path, outputs
         finally:
             if stream is not None:
                 stream.close()
@@ -309,13 +325,16 @@ class ReverbASR:
                    verbatimicity: float = 1.0, chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
                    decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                    simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
-                   length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None) -> str:
+                   length_penalty: float = 0.0, timings_adjustment: float = 230, context_graph=None,
+                   diarization=None) -> str:
+        """format: "txt", "ctm", or "stm" with `diarization` (speaker-attributed words, see transcribe_files)."""
         return self.transcribe_modes(
             audio_file, modes=[mode], format=format, verbatimicity=verbatimicity, chunk_size=chunk_size,
             batch_size=batch_size, beam_size=beam_size, decoding_chunk_size=decoding_chunk_size,
             num_decoding_left_chunks=num_decoding_left_chunks, ctc_weight=ctc_weight,
             simulate_streaming=simulate_streaming, reverse_weight=reverse_weight, blank_penalty=blank_penalty,
-            length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph)[0]
+            length_penalty=length_penalty, timings_adjustment=timings_adjustment, context_graph=context_graph,
+            diarization=diarization)[0]
 
     def context_graph(self, phrases, score: float = 6.0) -> ContextGraph:
         """A context biasing graph over `phrases` — a file with one phrase per line, or a list of strings — tokenized
@@ -486,6 +505,17 @@ def get_output(format: str, tokenizer, audio_name: str, hyps: List[DecodeResult]
         time_shift_ms += chunk_size * input_frame_length
         lines.extend(render(words))
     return delimiter.join(lines)
+
+
+def speaker_outputs(diarization, audio_file, ctms: List[str]) -> Tuple[str, List[str]]:
+    """Diarizes `audio_file` -> (its RTTM as diarization.infer writes it, [the STM words2speakers writes from each
+    CTM]).  The turns and words round-trip through the RTTM and CTM text, so the STM is the file chain's."""
+    import os
+    from .diarization.infer import read_audio
+    from .diarization.words2speakers import rttm_text, stm_text
+    uri = os.path.splitext(os.path.basename(str(audio_file)))[0]
+    rttm = rttm_text(uri, diarization(read_audio(str(audio_file))))
+    return rttm, [stm_text(uri, rttm, ctm) for ctm in ctms]
 
 
 def load_model(model: str, gpu: int = -1, precision: str | None = None) -> ReverbASR:
