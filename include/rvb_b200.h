@@ -65,6 +65,9 @@ typedef struct rvb_model_config {
 RVB_API const char* rvb_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process */
 RVB_API unsigned long long rvb_launch_count(void);
+/* bytes this library currently holds in the workspaces and weights of its models: device memory and page-locked
+ * host memory, over every model and thread of the process */
+RVB_API int rvb_held_bytes(long long* device, long long* pinned);
 /* 0 = wgmma/TMA GEMM (default), 1 = plain CUDA-core bring-up GEMM (debug only), 2 = wgmma GEMM with 64-wide tiles */
 RVB_API int rvb_set_gemm_impl(int impl);
 RVB_API int rvb_get_gemm_impl(void);

@@ -41,6 +41,7 @@ _vp, _i, _f, _ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
 SIGNATURES = {
     "rvb_last_error": (C.c_char_p, []),
     "rvb_launch_count": (C.c_ulonglong, []),
+    "rvb_held_bytes": (_i, [_vp, _vp]),
     "rvb_set_gemm_impl": (_i, [_i]),
     "rvb_get_gemm_impl": (_i, []),
     "rvb_gemm_profile_begin": (_i, []),

@@ -38,7 +38,7 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     objdir = os.path.join(CSRC, "build")
     os.makedirs(objdir, exist_ok=True)
-    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "kernels.h")] + \
+    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "kernels.h", "host_mem.h")] + \
               [os.path.join(HERE, "..", "include", h) for h in ("rvb_b200.h", "rvb_diar.h")]
     nvcc = _nvcc()
 

@@ -17,35 +17,14 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/rvb_diar.h"
+#include "host_mem.h"
 #include "kernels.h"
 
 namespace rvb {
-
-struct EBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    RVB_CHECK_CUDA(cudaMalloc(&p, bytes + 256));
-    cap = bytes + 256;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-  template <typename T>
-  T* as() const { return reinterpret_cast<T*>(p); }
-};
 
 __global__ void scale_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, float s) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -210,8 +189,7 @@ struct ConvW {
 struct rvb_emb_model {
   rvb_emb_config cfg;
   bool finalized = false;
-  std::map<std::string, std::vector<float>> host;
-  std::vector<void*> allocs;
+  rvb::WeightStore store{"rvb_emb_finalize:"};
   float* in_w = nullptr;   // (C, 9) fp32, BN folded
   float* in_b = nullptr;
   struct Block {
@@ -221,36 +199,16 @@ struct rvb_emb_model {
   std::vector<Block> blocks;
   float* seg_w = nullptr;
   float* seg_b = nullptr;
-  rvb::EBuf ws_wave, ws_feat, ws_x, ws_a0, ws_a1, ws_a2, ws_col, ws_y, ws_stats;
+  rvb::DevBuf ws_wave, ws_feat, ws_x, ws_a0, ws_a1, ws_a2, ws_col, ws_y, ws_stats;
 };
 
 namespace rvb {
 
-static int emb_alloc(rvb_emb_model* m, size_t bytes, void** out) {
-  RVB_CHECK_CUDA(cudaMalloc(out, bytes));
-  m->allocs.push_back(*out);
-  return 0;
-}
-static int emb_upload_f32(rvb_emb_model* m, const float* h, size_t n, float** out) {
-  void* p = nullptr;
-  if (emb_alloc(m, n * sizeof(float), &p)) return -1;
-  RVB_CHECK_CUDA(cudaMemcpy(p, h, n * sizeof(float), cudaMemcpyHostToDevice));
-  *out = reinterpret_cast<float*>(p);
-  return 0;
-}
-static int emb_need(rvb_emb_model* m, const std::string& name, size_t n, const std::vector<float>** out) {
-  auto it = m->host.find(name);
-  RVB_REQUIRE(it != m->host.end(), "rvb_emb_finalize: tensor '%s' was not provided", name.c_str());
-  RVB_REQUIRE(it->second.size() == n, "rvb_emb_finalize: tensor '%s' has %zu elements, expected %zu", name.c_str(),
-              it->second.size(), n);
-  *out = &it->second;
-  return 0;
-}
 // BatchNorm2d (eval) folded into the convolution before it: scale[c] = gamma / sqrt(var + eps), shift = beta - mean * scale
 static int emb_bn(rvb_emb_model* m, const std::string& p, int C, std::vector<float>* scale, std::vector<float>* shift) {
   const std::vector<float>*g, *b, *mu, *var;
-  if (emb_need(m, p + ".weight", C, &g) || emb_need(m, p + ".bias", C, &b) || emb_need(m, p + ".running_mean", C, &mu) ||
-      emb_need(m, p + ".running_var", C, &var))
+  if (m->store.need(p + ".weight", C, &g) || m->store.need(p + ".bias", C, &b) ||
+      m->store.need(p + ".running_mean", C, &mu) || m->store.need(p + ".running_var", C, &var))
     return -1;
   scale->resize(C);
   shift->resize(C);
@@ -265,7 +223,7 @@ static int emb_bn(rvb_emb_model* m, const std::string& p, int C, std::vector<flo
 static int emb_conv(rvb_emb_model* m, const std::string& wname, const std::string& bnname, int cin, int cout, int ks,
                     int stride, ConvW* out) {
   const std::vector<float>* w;
-  if (emb_need(m, wname, (size_t)cout * cin * ks * ks, &w)) return -1;
+  if (m->store.need(wname, (size_t)cout * cin * ks * ks, &w)) return -1;
   std::vector<float> scale, shift;
   if (emb_bn(m, bnname, cout, &scale, &shift)) return -1;
   const int K = ks * ks * cin;
@@ -276,11 +234,9 @@ static int emb_conv(rvb_emb_model* m, const std::string& wname, const std::strin
         for (int kw = 0; kw < ks; ++kw)
           packed[(size_t)co * K + (kh * ks + kw) * cin + ci] =
               __float2bfloat16((*w)[(((size_t)co * cin + ci) * ks + kh) * ks + kw] * scale[co]);
-  void* p = nullptr;
-  if (emb_alloc(m, packed.size() * sizeof(bf16), &p)) return -1;
-  RVB_CHECK_CUDA(cudaMemcpy(p, packed.data(), packed.size() * sizeof(bf16), cudaMemcpyHostToDevice));
-  out->w = reinterpret_cast<bf16*>(p);
-  if (emb_upload_f32(m, shift.data(), shift.size(), &out->b)) return -1;
+  if (m->store.upload(packed.data(), packed.size(), &out->w) ||
+      m->store.upload(shift.data(), shift.size(), &out->b))
+    return -1;
   out->cin = cin;
   out->cout = cout;
   out->ks = ks;
@@ -344,7 +300,7 @@ RVB_API rvb_emb_model* rvb_emb_create(const rvb_emb_config* cfg) {
 RVB_API int rvb_emb_set_tensor(rvb_emb_model* m, const char* name, const float* host, long long count) {
   RVB_REQUIRE(m && name && host && count > 0, "rvb_emb_set_tensor: bad arguments");
   RVB_REQUIRE(!m->finalized, "rvb_emb_set_tensor: model already finalized");
-  m->host[name].assign(host, host + count);
+  m->store.set(name, host, (size_t)count);
   return 0;
 }
 
@@ -355,13 +311,13 @@ RVB_API int rvb_emb_finalize(rvb_emb_model* m) {
   const int C0 = c.m_channels;
   {
     const std::vector<float>* w;
-    if (emb_need(m, "resnet.conv1.weight", (size_t)C0 * 9, &w)) return -1;
+    if (m->store.need("resnet.conv1.weight", (size_t)C0 * 9, &w)) return -1;
     std::vector<float> scale, shift;
     if (emb_bn(m, "resnet.bn1", C0, &scale, &shift)) return -1;
     std::vector<float> wf((size_t)C0 * 9);
     for (int co = 0; co < C0; ++co)
       for (int k = 0; k < 9; ++k) wf[(size_t)co * 9 + k] = (*w)[(size_t)co * 9 + k] * scale[co];
-    if (emb_upload_f32(m, wf.data(), wf.size(), &m->in_w) || emb_upload_f32(m, shift.data(), shift.size(), &m->in_b))
+    if (m->store.upload(wf.data(), wf.size(), &m->in_w) || m->store.upload(shift.data(), shift.size(), &m->in_b))
       return -1;
   }
   int cin = C0;
@@ -382,19 +338,18 @@ RVB_API int rvb_emb_finalize(rvb_emb_model* m) {
   const int Fq = conv_out(conv_out(conv_out(c.num_mel_bins, 2), 2), 2);
   const int D = cin * Fq;
   const std::vector<float>* t;
-  if (emb_need(m, "resnet.seg_1.weight", (size_t)c.embed_dim * 2 * D, &t) || emb_upload_f32(m, t->data(), t->size(), &m->seg_w))
+  if (m->store.need("resnet.seg_1.weight", (size_t)c.embed_dim * 2 * D, &t) ||
+      m->store.upload(t->data(), t->size(), &m->seg_w))
     return -1;
-  if (emb_need(m, "resnet.seg_1.bias", c.embed_dim, &t) || emb_upload_f32(m, t->data(), t->size(), &m->seg_b)) return -1;
-  m->host.clear();
+  if (m->store.need("resnet.seg_1.bias", c.embed_dim, &t) || m->store.upload(t->data(), t->size(), &m->seg_b))
+    return -1;
+  m->store.drop_host();
   m->finalized = true;
   return 0;
 }
 
 RVB_API void rvb_emb_destroy(rvb_emb_model* m) {
   if (!m) return;
-  for (void* p : m->allocs) cudaFree(p);
-  for (rvb::EBuf* b : {&m->ws_wave, &m->ws_feat, &m->ws_x, &m->ws_a0, &m->ws_a1, &m->ws_a2, &m->ws_col, &m->ws_y, &m->ws_stats})
-    b->release();
   delete m;
 }
 

@@ -22,35 +22,14 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/rvb_diar.h"
+#include "host_mem.h"
 #include "kernels.h"
 
 namespace rvb {
-
-struct DBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    RVB_CHECK_CUDA(cudaMalloc(&p, bytes + 256));
-    cap = bytes + 256;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-  template <typename T>
-  T* as() const { return reinterpret_cast<T*>(p); }
-};
 
 // ------------------------------------------------------------------------------------------------ small reductions
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -353,8 +332,7 @@ __global__ void logsoftmax_rows_kernel(const float* __restrict__ x, float* __res
 struct rvb_seg_model {
   rvb_seg_config cfg;
   bool finalized = false;
-  std::map<std::string, std::vector<float>> host;
-  std::vector<void*> allocs;
+  rvb::WeightStore store{"rvb_seg_finalize:"};
   float wav_w = 1.f, wav_b = 0.f;
   float* filt = nullptr;
   float* norm_w[3] = {nullptr, nullptr, nullptr};
@@ -365,28 +343,10 @@ struct rvb_seg_model {
   std::vector<float*> lin_w, lin_b;
   float* cls_w = nullptr;
   float* cls_b = nullptr;
-  rvb::DBuf ws_a, ws_b, ws_g, ws_h0, ws_h1;
+  rvb::DevBuf ws_a, ws_b, ws_g, ws_h0, ws_h1;
 };
 
 namespace rvb {
-
-static int seg_upload(rvb_seg_model* m, const float* h, size_t n, float** out) {
-  void* p = nullptr;
-  RVB_CHECK_CUDA(cudaMalloc(&p, n * sizeof(float)));
-  m->allocs.push_back(p);
-  RVB_CHECK_CUDA(cudaMemcpy(p, h, n * sizeof(float), cudaMemcpyHostToDevice));
-  *out = reinterpret_cast<float*>(p);
-  return 0;
-}
-
-static int seg_need(rvb_seg_model* m, const std::string& name, size_t n, const std::vector<float>** out) {
-  auto it = m->host.find(name);
-  RVB_REQUIRE(it != m->host.end(), "rvb_seg_finalize: tensor '%s' was not provided", name.c_str());
-  RVB_REQUIRE(it->second.size() == n, "rvb_seg_finalize: tensor '%s' has %zu elements, expected %zu", name.c_str(),
-              it->second.size(), n);
-  *out = &it->second;
-  return 0;
-}
 
 // ParamSincFB.filters() (asteroid-filterbanks): cosine and sine band-pass filters with a mirrored half Hamming window
 static void sinc_filter_bank(const std::vector<float>& low_hz_, const std::vector<float>& band_hz_, int kernel,
@@ -455,7 +415,7 @@ RVB_API rvb_seg_model* rvb_seg_create(const rvb_seg_config* cfg) {
 RVB_API int rvb_seg_set_tensor(rvb_seg_model* m, const char* name, const float* host, long long count) {
   RVB_REQUIRE(m && name && host && count > 0, "rvb_seg_set_tensor: bad arguments");
   RVB_REQUIRE(!m->finalized, "rvb_seg_set_tensor: model already finalized");
-  m->host[name].assign(host, host + count);
+  m->store.set(name, host, (size_t)count);
   return 0;
 }
 
@@ -465,30 +425,31 @@ RVB_API int rvb_seg_finalize(rvb_seg_model* m) {
   const rvb_seg_config& c = m->cfg;
   const std::vector<float>* t = nullptr;
   const std::vector<float>* t2 = nullptr;
-  if (seg_need(m, "sincnet.wav_norm1d.weight", 1, &t)) return -1;
+  if (m->store.need("sincnet.wav_norm1d.weight", 1, &t)) return -1;
   m->wav_w = (*t)[0];
-  if (seg_need(m, "sincnet.wav_norm1d.bias", 1, &t)) return -1;
+  if (m->store.need("sincnet.wav_norm1d.bias", 1, &t)) return -1;
   m->wav_b = (*t)[0];
   const int half = c.sinc_filters / 2;
-  if (seg_need(m, "sincnet.conv1d.0.filterbank.low_hz_", half, &t) ||
-      seg_need(m, "sincnet.conv1d.0.filterbank.band_hz_", half, &t2))
+  if (m->store.need("sincnet.conv1d.0.filterbank.low_hz_", half, &t) ||
+      m->store.need("sincnet.conv1d.0.filterbank.band_hz_", half, &t2))
     return -1;
   std::vector<float> bank;
   sinc_filter_bank(*t, *t2, c.sinc_kernel, (double)c.sample_rate, &bank);
-  if (seg_upload(m, bank.data(), bank.size(), &m->filt)) return -1;
+  if (m->store.upload(bank.data(), bank.size(), &m->filt)) return -1;
   const int nch[3] = {c.sinc_filters, c.conv_channels, c.conv_channels};
   for (int i = 0; i < 3; ++i) {
     const std::string p = "sincnet.norm1d." + std::to_string(i);
-    if (seg_need(m, p + ".weight", nch[i], &t) || seg_upload(m, t->data(), t->size(), &m->norm_w[i])) return -1;
-    if (seg_need(m, p + ".bias", nch[i], &t) || seg_upload(m, t->data(), t->size(), &m->norm_b[i])) return -1;
+    if (m->store.need(p + ".weight", nch[i], &t) || m->store.upload(t->data(), t->size(), &m->norm_w[i])) return -1;
+    if (m->store.need(p + ".bias", nch[i], &t) || m->store.upload(t->data(), t->size(), &m->norm_b[i])) return -1;
   }
   for (int i = 0; i < 2; ++i) {
     const std::string p = "sincnet.conv1d." + std::to_string(i + 1);
     const int cin = nch[i];
-    if (seg_need(m, p + ".weight", (size_t)c.conv_channels * cin * c.conv_kernel, &t) ||
-        seg_upload(m, t->data(), t->size(), &m->conv_w[i]))
+    if (m->store.need(p + ".weight", (size_t)c.conv_channels * cin * c.conv_kernel, &t) ||
+        m->store.upload(t->data(), t->size(), &m->conv_w[i]))
       return -1;
-    if (seg_need(m, p + ".bias", c.conv_channels, &t) || seg_upload(m, t->data(), t->size(), &m->conv_b[i])) return -1;
+    if (m->store.need(p + ".bias", c.conv_channels, &t) || m->store.upload(t->data(), t->size(), &m->conv_b[i]))
+      return -1;
   }
   const int H = c.lstm_hidden;
   for (int l = 0; l < c.lstm_layers; ++l) {
@@ -496,17 +457,18 @@ RVB_API int rvb_seg_finalize(rvb_seg_model* m) {
     std::vector<float> wih((size_t)2 * 4 * H * in), whh((size_t)2 * 4 * H * H), bias((size_t)2 * 4 * H);
     for (int d = 0; d < 2; ++d) {
       const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
-      if (seg_need(m, "lstm.weight_ih" + sfx, (size_t)4 * H * in, &t)) return -1;
+      if (m->store.need("lstm.weight_ih" + sfx, (size_t)4 * H * in, &t)) return -1;
       memcpy(wih.data() + (size_t)d * 4 * H * in, t->data(), t->size() * sizeof(float));
-      if (seg_need(m, "lstm.weight_hh" + sfx, (size_t)4 * H * H, &t)) return -1;
+      if (m->store.need("lstm.weight_hh" + sfx, (size_t)4 * H * H, &t)) return -1;
       memcpy(whh.data() + (size_t)d * 4 * H * H, t->data(), t->size() * sizeof(float));
-      if (seg_need(m, "lstm.bias_ih" + sfx, (size_t)4 * H, &t) || seg_need(m, "lstm.bias_hh" + sfx, (size_t)4 * H, &t2))
+      if (m->store.need("lstm.bias_ih" + sfx, (size_t)4 * H, &t) ||
+          m->store.need("lstm.bias_hh" + sfx, (size_t)4 * H, &t2))
         return -1;
       for (int i = 0; i < 4 * H; ++i) bias[(size_t)d * 4 * H + i] = (*t)[i] + (*t2)[i];
     }
     float *a = nullptr, *b = nullptr, *cc = nullptr;
-    if (seg_upload(m, wih.data(), wih.size(), &a) || seg_upload(m, whh.data(), whh.size(), &b) ||
-        seg_upload(m, bias.data(), bias.size(), &cc))
+    if (m->store.upload(wih.data(), wih.size(), &a) || m->store.upload(whh.data(), whh.size(), &b) ||
+        m->store.upload(bias.data(), bias.size(), &cc))
       return -1;
     m->wih.push_back(a);
     m->whh.push_back(b);
@@ -516,24 +478,25 @@ RVB_API int rvb_seg_finalize(rvb_seg_model* m) {
   for (int i = 0; i < c.linear_layers; ++i) {
     const std::string p = "linear." + std::to_string(i);
     float *a = nullptr, *b = nullptr;
-    if (seg_need(m, p + ".weight", (size_t)c.linear_dim * in, &t) || seg_upload(m, t->data(), t->size(), &a)) return -1;
-    if (seg_need(m, p + ".bias", c.linear_dim, &t) || seg_upload(m, t->data(), t->size(), &b)) return -1;
+    if (m->store.need(p + ".weight", (size_t)c.linear_dim * in, &t) || m->store.upload(t->data(), t->size(), &a))
+      return -1;
+    if (m->store.need(p + ".bias", c.linear_dim, &t) || m->store.upload(t->data(), t->size(), &b)) return -1;
     m->lin_w.push_back(a);
     m->lin_b.push_back(b);
     in = c.linear_dim;
   }
-  if (seg_need(m, "classifier.weight", (size_t)c.num_classes * in, &t) || seg_upload(m, t->data(), t->size(), &m->cls_w))
+  if (m->store.need("classifier.weight", (size_t)c.num_classes * in, &t) ||
+      m->store.upload(t->data(), t->size(), &m->cls_w))
     return -1;
-  if (seg_need(m, "classifier.bias", c.num_classes, &t) || seg_upload(m, t->data(), t->size(), &m->cls_b)) return -1;
-  m->host.clear();
+  if (m->store.need("classifier.bias", c.num_classes, &t) || m->store.upload(t->data(), t->size(), &m->cls_b))
+    return -1;
+  m->store.drop_host();
   m->finalized = true;
   return 0;
 }
 
 RVB_API void rvb_seg_destroy(rvb_seg_model* m) {
   if (!m) return;
-  for (void* p : m->allocs) cudaFree(p);
-  for (rvb::DBuf* b : {&m->ws_a, &m->ws_b, &m->ws_g, &m->ws_h0, &m->ws_h1}) b->release();
   delete m;
 }
 

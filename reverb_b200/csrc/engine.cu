@@ -16,11 +16,12 @@
 
 #include <algorithm>
 #include <atomic>
-#include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/rvb_b200.h"
+#include "host_mem.h"
 #include "kernels.h"
 
 namespace rvb {
@@ -35,49 +36,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 const char* last_error() { return g_err; }
-
-struct DevBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = bytes + (bytes >> 3) + 256;
-    RVB_CHECK_CUDA(cudaMalloc(&p, want));
-    cap = want;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-  template <typename T>
-  T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-struct HostPinned {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-    RVB_CHECK_CUDA(cudaMallocHost(&p, bytes + 256));
-    cap = bytes + 256;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-  }
-  template <typename T>
-  T* as() const { return reinterpret_cast<T*>(p); }
-};
 
 static inline uint16_t f2bf(float f) {
   uint32_t u;
@@ -152,9 +110,6 @@ struct DecRows {
       return -1;
     return 0;
   }
-  void release() {
-    for (DevBuf* b : {&x, &n, &qkv, &att, &h, &ybf, &kv}) b->release();
-  }
 };
 
 // The n-best of a CTC prefix beam search over B utterances, `beam` hypothesis slots each, in one device buffer and a
@@ -194,23 +149,11 @@ struct NBest {
     len_cap = len_cap_;
     return (dev.ensure(bytes()) || host.ensure(bytes())) ? -1 : 0;
   }
-  void release() {
-    dev.release();
-    host.release();
-  }
 };
 
-}  // namespace rvb
-
-using namespace rvb;
-
-struct rvb_model {
-  rvb_model_config cfg;
-  std::map<std::string, std::vector<float>> host;  // raw reference tensors until finalize
-  bool finalized = false;
-  std::vector<void*> owned;  // device allocations owned by the plan
-
-  // encoder
+// The packed weights of a plan, uploaded by rvb_model_finalize into the plan's WeightStore.  A fork copies them and
+// replaces only the folded language-specific linears (EncLayer::lang, DecLayer::lang) by its own.
+struct Weights {
   float* cmvn_mean = nullptr;
   float* cmvn_istd = nullptr;
   float* conv1_w = nullptr;  // (d, 9)
@@ -222,6 +165,17 @@ struct rvb_model {
   Norm after_norm;
   Linear ctc;
   Decoder dec_l, dec_r;
+};
+
+}  // namespace rvb
+
+using namespace rvb;
+
+struct rvb_model {
+  rvb_model_config cfg;
+  WeightStore store{"model:"};  // raw reference tensors until finalize, and the device allocations of this plan
+  bool finalized = false;
+  Weights w;
   std::vector<float> cur_cat;  // cat_embs the LSL folds were computed for
   bool x3 = false;             // cfg.precision == 1: bf16x3 "fp32-accurate" mode (GemmArgs::x3, kernels.h)
   int pm() const { return x3 ? 2 : 1; }  // physical width multiplier of every bf16 operand ([hi | lo] pairs)
@@ -243,94 +197,48 @@ struct rvb_model {
   int lens_slot = 0;
   int lens_cap = 0;             // batch rows per slot of the pinned length ring (the largest B seen)
   static constexpr int kTickets = 4;
-  rvb::SearchTicket* tickets = nullptr;  // [kTickets], created on first use (engine.cu search_submit)
-  rvb::DecCache* dcache = nullptr;        // KV cache of the autoregressive decoder (decoder_cache_begin / _step)
-  cudaStream_t s_search = nullptr;        // side stream of the prefix beam search (search_submit)
+  std::unique_ptr<rvb::SearchTicket[]> tickets;  // [kTickets], created on first use (search_submit_any)
+  std::unique_ptr<rvb::DecCache> dcache;         // KV cache of the autoregressive decoder (decoder_cache_begin / _step)
+  cudaStream_t s_search = nullptr;               // side stream of the prefix beam search (search_submit)
   cudaEvent_t ev_topk = nullptr;
 
+  ~rvb_model();
   int F1() const { return (cfg.input_dim - 1) / 2; }
   int F2() const { return (F1() - 1) / 2; }
 };
 
 namespace rvb {
 
-static const std::vector<float>* find_host(rvb_model* m, const std::string& name) {
-  auto it = m->host.find(name);
-  return it == m->host.end() ? nullptr : &it->second;
-}
-
-static int need(rvb_model* m, const std::string& name, size_t numel, const std::vector<float>** out) {
-  const std::vector<float>* v = find_host(m, name);
-  RVB_REQUIRE(v != nullptr, "model: tensor '%s' was not provided", name.c_str());
-  RVB_REQUIRE(v->size() == numel, "model: tensor '%s' has %zu elements, expected %zu", name.c_str(), v->size(), numel);
-  *out = v;
-  return 0;
-}
-
-static int upload_f32(rvb_model* m, const float* src, size_t n, float** dst) {
-  void* p = nullptr;
-  RVB_CHECK_CUDA(cudaMalloc(&p, n * sizeof(float) + 16));
-  RVB_CHECK_CUDA(cudaMemcpy(p, src, n * sizeof(float), cudaMemcpyHostToDevice));
-  m->owned.push_back(p);
-  *dst = reinterpret_cast<float*>(p);
-  return 0;
-}
-
-static int upload_bf16(rvb_model* m, const float* src, size_t n, bf16** dst) {
-  std::vector<uint16_t> tmp(n);
-  for (size_t i = 0; i < n; ++i) tmp[i] = f2bf(src[i]);
-  void* p = nullptr;
-  RVB_CHECK_CUDA(cudaMalloc(&p, n * sizeof(uint16_t) + 16));
-  RVB_CHECK_CUDA(cudaMemcpy(p, tmp.data(), n * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  m->owned.push_back(p);
-  *dst = reinterpret_cast<bf16*>(p);
-  return 0;
-}
-
 // GEMM weight (N, K) fp32 -> device bf16 (N, K), or the pair layout (N, 2K) = [hi | lo] in the accurate mode
 static int upload_w(rvb_model* m, const float* src, size_t N, size_t K, bf16** dst) {
-  if (!m->x3) return upload_bf16(m, src, N * K, dst);
-  std::vector<uint16_t> tmp(N * K * 2);
+  const size_t pm = m->pm();
+  std::vector<uint16_t> tmp(N * K * pm);
   for (size_t n = 0; n < N; ++n)
     for (size_t k = 0; k < K; ++k) {
       const float v = src[n * K + k];
       const uint16_t h = f2bf(v);
-      tmp[n * 2 * K + k] = h;
-      tmp[n * 2 * K + K + k] = f2bf(v - bf2f(h));
+      tmp[n * pm * K + k] = h;
+      if (pm == 2) tmp[n * pm * K + K + k] = f2bf(v - bf2f(h));
     }
-  void* p = nullptr;
-  RVB_CHECK_CUDA(cudaMalloc(&p, tmp.size() * sizeof(uint16_t) + 16));
-  RVB_CHECK_CUDA(cudaMemcpy(p, tmp.data(), tmp.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  m->owned.push_back(p);
-  *dst = reinterpret_cast<bf16*>(p);
-  return 0;
-}
-
-static int alloc_dev(rvb_model* m, size_t bytes, void** dst) {
-  void* p = nullptr;
-  RVB_CHECK_CUDA(cudaMalloc(&p, bytes + 16));
-  RVB_CHECK_CUDA(cudaMemset(p, 0, bytes + 16));
-  m->owned.push_back(p);
-  *dst = p;
-  return 0;
+  return m->store.upload(tmp.data(), tmp.size(), dst);
 }
 
 // nn.Linear `prefix`.{weight,bias}; bias optional (zeros when absent and `bias_optional`)
 static int load_linear(rvb_model* m, const std::string& prefix, int N, int K, Linear* out, bool has_bias = true,
                        bool bias_optional = false) {
   const std::vector<float>* w;
-  if (need(m, prefix + ".weight", (size_t)N * K, &w)) return -1;
+  if (m->store.need(prefix + ".weight", (size_t)N * K, &w)) return -1;
   if (upload_w(m, w->data(), N, K, &out->w)) return -1;
   out->N = N;
   out->K = K;
   if (has_bias) {
-    const std::vector<float>* b = find_host(m, prefix + ".bias");
+    const std::vector<float>* b = m->store.find(prefix + ".bias");
     if (b == nullptr && bias_optional) {
       std::vector<float> z(N, 0.f);
-      if (upload_f32(m, z.data(), N, &out->b)) return -1;
+      if (m->store.upload(z.data(), N, &out->b)) return -1;
     } else {
-      if (need(m, prefix + ".bias", N, &b)) return -1;
-      if (upload_f32(m, b->data(), N, &out->b)) return -1;
+      if (m->store.need(prefix + ".bias", N, &b)) return -1;
+      if (m->store.upload(b->data(), N, &out->b)) return -1;
     }
   }
   return 0;
@@ -342,7 +250,8 @@ static int load_linear(rvb_model* m, const std::string& prefix, int N, int K, Li
 static int load_linear_glu(rvb_model* m, const std::string& prefix, int C, int K, Linear* out, float** pad_glu) {
   const std::vector<float>*w, *b;
   RVB_REQUIRE(C % 32 == 0, "model: conv module channels (%d) must be a multiple of 32", C);
-  if (need(m, prefix + ".weight", (size_t)2 * C * K, &w) || need(m, prefix + ".bias", (size_t)2 * C, &b)) return -1;
+  if (m->store.need(prefix + ".weight", (size_t)2 * C * K, &w) || m->store.need(prefix + ".bias", (size_t)2 * C, &b))
+    return -1;
   std::vector<float> pw((size_t)2 * C * K), pb((size_t)2 * C), pad(C);
   for (int c = 0; c < C; ++c) {
     const int ra = 64 * (c / 32) + (c % 32), rg = ra + 32;
@@ -353,8 +262,8 @@ static int load_linear_glu(rvb_model* m, const std::string& prefix, int C, int K
     const float g = (*b)[c] / (1.f + expf(-(*b)[C + c]));
     pad[c] = m->x3 ? g : bf2f(f2bf(g));  // the engine stores GLU outputs as bf16 (a hi/lo pair in the accurate mode)
   }
-  if (upload_w(m, pw.data(), (size_t)2 * C, K, &out->w) || upload_f32(m, pb.data(), pb.size(), &out->b) ||
-      upload_f32(m, pad.data(), pad.size(), pad_glu))
+  if (upload_w(m, pw.data(), (size_t)2 * C, K, &out->w) || m->store.upload(pb.data(), pb.size(), &out->b) ||
+      m->store.upload(pad.data(), pad.size(), pad_glu))
     return -1;
   out->N = 2 * C;
   out->K = K;
@@ -363,8 +272,8 @@ static int load_linear_glu(rvb_model* m, const std::string& prefix, int C, int K
 
 static int load_norm(rvb_model* m, const std::string& prefix, int d, Norm* out) {
   const std::vector<float>*g, *b;
-  if (need(m, prefix + ".weight", d, &g) || need(m, prefix + ".bias", d, &b)) return -1;
-  if (upload_f32(m, g->data(), d, &out->g) || upload_f32(m, b->data(), d, &out->b)) return -1;
+  if (m->store.need(prefix + ".weight", d, &g) || m->store.need(prefix + ".bias", d, &b)) return -1;
+  if (m->store.upload(g->data(), d, &out->g) || m->store.upload(b->data(), d, &out->b)) return -1;
   return 0;
 }
 
@@ -374,9 +283,9 @@ static int load_fused(rvb_model* m, const std::string& prefix, const std::vector
   std::vector<float> w, b;
   for (const auto& part : parts) {
     const std::vector<float>* pw;
-    if (need(m, prefix + "." + part + ".weight", (size_t)d * d, &pw)) return -1;
+    if (m->store.need(prefix + "." + part + ".weight", (size_t)d * d, &pw)) return -1;
     w.insert(w.end(), pw->begin(), pw->end());
-    const std::vector<float>* pb = find_host(m, prefix + "." + part + ".bias");
+    const std::vector<float>* pb = m->store.find(prefix + "." + part + ".bias");
     if (pb) {
       RVB_REQUIRE(pb->size() == (size_t)d, "model: bad bias size for %s.%s", prefix.c_str(), part.c_str());
       b.insert(b.end(), pb->begin(), pb->end());
@@ -384,9 +293,19 @@ static int load_fused(rvb_model* m, const std::string& prefix, const std::vector
       b.insert(b.end(), d, 0.f);  // key_bias = False
     }
   }
-  if (upload_w(m, w.data(), (size_t)d * parts.size(), d, &out->w) || upload_f32(m, b.data(), b.size(), &out->b)) return -1;
+  if (upload_w(m, w.data(), (size_t)d * parts.size(), d, &out->w) || m->store.upload(b.data(), b.size(), &out->b))
+    return -1;
   out->N = d * (int)parts.size();
   out->K = d;
+  return 0;
+}
+
+// zeroed device space of a language-specific linear that fold_lang fills for the current cat_embs
+static int alloc_fold(rvb_model* m, Linear* folded) {
+  const int d = m->cfg.d_model;
+  if (m->store.alloc_zeroed((size_t)d * d * m->pm(), &folded->w) || m->store.alloc_zeroed(d, &folded->b)) return -1;
+  folded->N = d;
+  folded->K = d;
   return 0;
 }
 
@@ -395,20 +314,13 @@ static int load_lang(rvb_model* m, const std::string& prefix, int d, int n_lang,
   for (int i = 0; i < n_lang; ++i) {
     const std::vector<float>*w, *b;
     std::string p = prefix + ".language_layers." + std::to_string(i);
-    if (need(m, p + ".weight", (size_t)d * d, &w) || need(m, p + ".bias", d, &b)) return -1;
+    if (m->store.need(p + ".weight", (size_t)d * d, &w) || m->store.need(p + ".bias", d, &b)) return -1;
     float *dw, *db;
-    if (upload_f32(m, w->data(), w->size(), &dw) || upload_f32(m, b->data(), d, &db)) return -1;
+    if (m->store.upload(w->data(), w->size(), &dw) || m->store.upload(b->data(), d, &db)) return -1;
     lw->push_back(dw);
     lb->push_back(db);
   }
-  void* p;
-  if (alloc_dev(m, (size_t)d * d * sizeof(bf16) * m->pm(), &p)) return -1;
-  folded->w = reinterpret_cast<bf16*>(p);
-  if (alloc_dev(m, (size_t)d * sizeof(float), &p)) return -1;
-  folded->b = reinterpret_cast<float*>(p);
-  folded->N = d;
-  folded->K = d;
-  return 0;
+  return alloc_fold(m, folded);
 }
 
 static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Decoder* dec) {
@@ -416,8 +328,8 @@ static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Deco
   const int d = c.d_model, V = c.vocab;
   const std::string p = "decoder." + side;
   const std::vector<float>* e;
-  if (need(m, p + ".embed.0.weight", (size_t)V * d, &e)) return -1;
-  if (upload_f32(m, e->data(), e->size(), &dec->emb)) return -1;
+  if (m->store.need(p + ".embed.0.weight", (size_t)V * d, &e)) return -1;
+  if (m->store.upload(e->data(), e->size(), &dec->emb)) return -1;
   if (load_norm(m, p + ".after_norm", d, &dec->after)) return -1;
   if (load_linear(m, p + ".output_layer", V, d, &dec->outl)) return -1;
   dec->layers.resize(nblocks);
@@ -449,43 +361,44 @@ static int finalize_model(rvb_model* m) {
   RVB_REQUIRE(d % 64 == 0, "model: d_model=%d must be a multiple of 64", d);
   RVB_REQUIRE(d % c.heads == 0 && d % c.dec_heads == 0, "model: heads must divide d_model");
   const std::vector<float>* t;
-  if (need(m, "encoder.global_cmvn.mean", F, &t) || upload_f32(m, t->data(), F, &m->cmvn_mean)) return -1;
-  if (need(m, "encoder.global_cmvn.istd", F, &t) || upload_f32(m, t->data(), F, &m->cmvn_istd)) return -1;
-  if (need(m, "encoder.embed.conv.0.weight", (size_t)d * 9, &t) || upload_f32(m, t->data(), t->size(), &m->conv1_w))
+  if (m->store.need("encoder.global_cmvn.mean", F, &t) || m->store.upload(t->data(), F, &m->w.cmvn_mean)) return -1;
+  if (m->store.need("encoder.global_cmvn.istd", F, &t) || m->store.upload(t->data(), F, &m->w.cmvn_istd)) return -1;
+  if (m->store.need("encoder.embed.conv.0.weight", (size_t)d * 9, &t) ||
+      m->store.upload(t->data(), t->size(), &m->w.conv1_w))
     return -1;
-  if (need(m, "encoder.embed.conv.0.bias", d, &t) || upload_f32(m, t->data(), d, &m->conv1_b)) return -1;
+  if (m->store.need("encoder.embed.conv.0.bias", d, &t) || m->store.upload(t->data(), d, &m->w.conv1_b)) return -1;
   {  // conv2 weight (o, c, kh, kw) -> (o, kh, kw, c)
-    if (need(m, "encoder.embed.conv.2.weight", (size_t)d * d * 9, &t)) return -1;
+    if (m->store.need("encoder.embed.conv.2.weight", (size_t)d * d * 9, &t)) return -1;
     std::vector<float> w((size_t)d * d * 9);
     for (int o = 0; o < d; ++o)
       for (int ci = 0; ci < d; ++ci)
         for (int k = 0; k < 9; ++k) w[((size_t)o * 9 + k) * d + ci] = (*t)[((size_t)o * d + ci) * 9 + k];
-    if (upload_w(m, w.data(), d, (size_t)9 * d, &m->conv2.w)) return -1;
-    if (need(m, "encoder.embed.conv.2.bias", d, &t) || upload_f32(m, t->data(), d, &m->conv2.b)) return -1;
-    m->conv2.N = d;
-    m->conv2.K = 9 * d;
+    if (upload_w(m, w.data(), d, (size_t)9 * d, &m->w.conv2.w)) return -1;
+    if (m->store.need("encoder.embed.conv.2.bias", d, &t) || m->store.upload(t->data(), d, &m->w.conv2.b)) return -1;
+    m->w.conv2.N = d;
+    m->w.conv2.K = 9 * d;
   }
   {  // embed linear (o, c*F2 + f) -> (o, f*d + c), times sqrt(d) (RelPositionalEncoding xscale, embedding.py:144)
-    if (need(m, "encoder.embed.out.0.weight", (size_t)d * d * F2, &t)) return -1;
+    if (m->store.need("encoder.embed.out.0.weight", (size_t)d * d * F2, &t)) return -1;
     const float xs = sqrtf((float)d);
     std::vector<float> w((size_t)d * d * F2);
     for (int o = 0; o < d; ++o)
       for (int ci = 0; ci < d; ++ci)
         for (int f = 0; f < F2; ++f)
           w[(size_t)o * d * F2 + (size_t)f * d + ci] = (*t)[(size_t)o * d * F2 + (size_t)ci * F2 + f] * xs;
-    if (upload_w(m, w.data(), d, (size_t)d * F2, &m->embed.w)) return -1;
-    if (need(m, "encoder.embed.out.0.bias", d, &t)) return -1;
+    if (upload_w(m, w.data(), d, (size_t)d * F2, &m->w.embed.w)) return -1;
+    if (m->store.need("encoder.embed.out.0.bias", d, &t)) return -1;
     std::vector<float> b(*t);
     for (auto& v : b) v *= xs;
-    if (upload_f32(m, b.data(), d, &m->embed.b)) return -1;
-    m->embed.N = d;
-    m->embed.K = d * F2;
+    if (m->store.upload(b.data(), d, &m->w.embed.b)) return -1;
+    m->w.embed.N = d;
+    m->w.embed.K = d * F2;
   }
-  if (load_norm(m, "encoder.after_norm", d, &m->after_norm)) return -1;
-  m->enc.resize(L);
+  if (load_norm(m, "encoder.after_norm", d, &m->w.after_norm)) return -1;
+  m->w.enc.resize(L);
   std::vector<float> posw;
   for (int i = 0; i < L; ++i) {
-    EncLayer& E = m->enc[i];
+    EncLayer& E = m->w.enc[i];
     const std::string p = "encoder.encoders." + std::to_string(i);
     E.lsl = c.num_langs > 0 && (i == 0 || i == L - 1);
     if (load_norm(m, p + ".norm_ff_macaron", d, &E.norm_ffm) || load_norm(m, p + ".norm_mha", d, &E.norm_mha) ||
@@ -499,35 +412,37 @@ static int finalize_model(rvb_model* m) {
       return -1;
     if (load_fused(m, p + ".self_attn", {"linear_q", "linear_k", "linear_v"}, d, &E.qkv)) return -1;
     if (load_linear(m, p + ".self_attn.linear_out", d, d, &E.out)) return -1;
-    if (need(m, p + ".self_attn.linear_pos.weight", (size_t)d * d, &t)) return -1;
+    if (m->store.need(p + ".self_attn.linear_pos.weight", (size_t)d * d, &t)) return -1;
     posw.insert(posw.end(), t->begin(), t->end());
-    if (need(m, p + ".self_attn.pos_bias_u", d, &t) || upload_f32(m, t->data(), d, &E.pos_u)) return -1;
-    if (need(m, p + ".self_attn.pos_bias_v", d, &t) || upload_f32(m, t->data(), d, &E.pos_v)) return -1;
+    if (m->store.need(p + ".self_attn.pos_bias_u", d, &t) || m->store.upload(t->data(), d, &E.pos_u)) return -1;
+    if (m->store.need(p + ".self_attn.pos_bias_v", d, &t) || m->store.upload(t->data(), d, &E.pos_v)) return -1;
     if (load_linear_glu(m, p + ".conv_module.pointwise_conv1", d, d, &E.pw1, &E.pad_glu) ||
         load_linear(m, p + ".conv_module.pointwise_conv2", d, d, &E.pw2))
       return -1;
-    if (need(m, p + ".conv_module.depthwise_conv.weight", (size_t)d * K, &t) ||
-        upload_f32(m, t->data(), t->size(), &E.dw_w))
+    if (m->store.need(p + ".conv_module.depthwise_conv.weight", (size_t)d * K, &t) ||
+        m->store.upload(t->data(), t->size(), &E.dw_w))
       return -1;
-    if (need(m, p + ".conv_module.depthwise_conv.bias", d, &t) || upload_f32(m, t->data(), d, &E.dw_b)) return -1;
+    if (m->store.need(p + ".conv_module.depthwise_conv.bias", d, &t) || m->store.upload(t->data(), d, &E.dw_b)) return -1;
     if (load_norm(m, p + ".conv_module.norm", d, &E.cnorm)) return -1;
     if (!c.cnn_layer_norm) {
-      if (need(m, p + ".conv_module.norm.running_mean", d, &t) || upload_f32(m, t->data(), d, &E.bn_mean)) return -1;
-      if (need(m, p + ".conv_module.norm.running_var", d, &t) || upload_f32(m, t->data(), d, &E.bn_var)) return -1;
+      if (m->store.need(p + ".conv_module.norm.running_mean", d, &t) || m->store.upload(t->data(), d, &E.bn_mean))
+        return -1;
+      if (m->store.need(p + ".conv_module.norm.running_var", d, &t) || m->store.upload(t->data(), d, &E.bn_var))
+        return -1;
     }
     if (E.lsl && load_lang(m, p, d, c.num_langs, &E.lang_w, &E.lang_b, &E.lang)) return -1;
   }
-  if (upload_w(m, posw.data(), (size_t)L * d, d, &m->pos_all.w)) return -1;
-  m->pos_all.N = L * d;
-  m->pos_all.K = d;
-  if (load_linear(m, "ctc.ctc_lo", c.vocab, d, &m->ctc)) return -1;
-  if (c.dec_blocks > 0 && find_host(m, "decoder.left_decoder.embed.0.weight")) {
-    if (load_decoder(m, "left_decoder", c.dec_blocks, &m->dec_l)) return -1;
+  if (upload_w(m, posw.data(), (size_t)L * d, d, &m->w.pos_all.w)) return -1;
+  m->w.pos_all.N = L * d;
+  m->w.pos_all.K = d;
+  if (load_linear(m, "ctc.ctc_lo", c.vocab, d, &m->w.ctc)) return -1;
+  if (c.dec_blocks > 0 && m->store.find("decoder.left_decoder.embed.0.weight")) {
+    if (load_decoder(m, "left_decoder", c.dec_blocks, &m->w.dec_l)) return -1;
   }
-  if (c.r_dec_blocks > 0 && find_host(m, "decoder.right_decoder.embed.0.weight")) {
-    if (load_decoder(m, "right_decoder", c.r_dec_blocks, &m->dec_r)) return -1;
+  if (c.r_dec_blocks > 0 && m->store.find("decoder.right_decoder.embed.0.weight")) {
+    if (load_decoder(m, "right_decoder", c.r_dec_blocks, &m->w.dec_r)) return -1;
   }
-  m->host.clear();
+  m->store.drop_host();
   m->finalized = true;
   return 0;
 }
@@ -549,9 +464,9 @@ static int fold_lang(rvb_model* m, const float* cat, int n_cat, cudaStream_t str
     if (launch_weighted_sum_bf16(lb.data(), cat, n_cat, d, nullptr, out.b, stream)) return -1;
     return 0;
   };
-  for (auto& E : m->enc)
+  for (auto& E : m->w.enc)
     if (E.lsl && fold(E.lang_w, E.lang_b, E.lang)) return -1;
-  for (Decoder* D : {&m->dec_l, &m->dec_r})
+  for (Decoder* D : {&m->w.dec_l, &m->w.dec_r})
     if (D->present)
       for (auto& Ld : D->layers)
         if (Ld.lsl && fold(Ld.lang_w, Ld.lang_b, Ld.lang)) return -1;
@@ -763,23 +678,24 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
   // ... where row t depends on t only (the GEMM computes rows independently): kept for the longest T' seen, and a
   // shorter batch reads its leading rows
   if (m->pall_T < Tp || m->pall_ptr != (const void*)pall) {
-    if (gemm(m, m->ws_pe.as<bf16>(), m->pos_all, Tp, ACT_NONE, OUT_BF16, pall, 1.f, stream, nullptr, 0, 0, false))
+    if (gemm(m, m->ws_pe.as<bf16>(), m->w.pos_all, Tp, ACT_NONE, OUT_BF16, pall, 1.f, stream, nullptr, 0, 0, false))
       return -1;
     m->pall_T = Tp;
     m->pall_ptr = pall;
   }
 
   // subsampling: CMVN + conv1 + ReLU ; conv2 + ReLU as implicit GEMM ; Linear(19 d -> d) * sqrt(d)
-  if (launch_conv1(d_feats, m->cmvn_mean, m->cmvn_istd, m->conv1_w, m->conv1_b, c1, B, T, F, d, T1, T1h, F1, stream, x3))
+  if (launch_conv1(d_feats, m->w.cmvn_mean, m->w.cmvn_istd, m->w.conv1_w, m->w.conv1_b, c1, B, T, F, d, T1, T1h, F1,
+                   stream, x3))
     return -1;
   {
     GemmArgs g;
     g.A = c1;
-    g.W = m->conv2.w;
+    g.W = m->w.conv2.w;
     g.M = (int)(M * F2);
     g.N = d;
     g.K = 9 * d;
-    g.bias = m->conv2.b;
+    g.bias = m->w.conv2.b;
     g.act = ACT_RELU;
     g.out_mode = OUT_BF16;
     g.out = c2;
@@ -798,15 +714,15 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     }
     if (launch_gemm(g, stream)) return -1;
   }
-  if (gemm(m, c2, m->embed, (int)M, ACT_NONE, OUT_F32, x, 1.f, stream)) return -1;
+  if (gemm(m, c2, m->w.embed, (int)M, ACT_NONE, OUT_F32, x, 1.f, stream)) return -1;
 
   const float att_scale = 1.0f / sqrtf((float)dk);
   // first pre-norm of block 0
-  if (launch_layernorm(x, m->enc[0].norm_ffm.g, m->enc[0].norm_ffm.b, 1e-5f, (int)M, d, n, nullptr, nullptr, 0, 0,
+  if (launch_layernorm(x, m->w.enc[0].norm_ffm.g, m->w.enc[0].norm_ffm.b, 1e-5f, (int)M, d, n, nullptr, nullptr, 0, 0,
                        stream, x3))
     return -1;
   for (int l = 0; l < L; ++l) {
-    EncLayer& E = m->enc[l];
+    EncLayer& E = m->w.enc[l];
     // macaron FFN: x += 0.5 * W2 SiLU(W1 n)                                   (encoder_layer.py:200-207)
     if (gemm(m, n, E.ffm1, (int)M, ACT_SILU, OUT_BF16, h, 1.f, stream)) return -1;
     if (gemm(m, h, E.ffm2, (int)M, ACT_NONE, OUT_RESID_F32, x, 0.5f, stream)) return -1;
@@ -932,7 +848,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     if (gemm(m, h, E.ff2, (int)M, ACT_NONE, OUT_RESID_F32, x, 0.5f, stream)) return -1;
     // x = norm_final(x) (+ y) ; then the next block's first pre-norm, or after_norm for the last block
     const bool last = (l == L - 1);
-    const Norm& nx = last ? m->after_norm : m->enc[l + 1].norm_ffm;
+    const Norm& nx = last ? m->w.after_norm : m->w.enc[l + 1].norm_ffm;
     if (launch_double_layernorm(x, E.norm_final.g, E.norm_final.b, E.lsl ? y : nullptr, x, nx.g, nx.b, 1e-5f, (int)M,
                                 d, last ? nullptr : n, last ? d_enc_out : nullptr, stream, x3))
       return -1;
@@ -963,7 +879,7 @@ static int ctc_topk(rvb_model* m, const float* d_enc_out, int B, int Tp, int k, 
   bf16* encbf;
   float* logits = m->ws_logits.as<float>();
   if (enc_operand(m, d_enc_out, M, &encbf, stream)) return -1;
-  if (gemm(m, encbf, m->ctc, (int)M, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
+  if (gemm(m, encbf, m->w.ctc, (int)M, ACT_NONE, OUT_F32, logits, 1.f, stream, nullptr, 0, ldv)) return -1;
   if (blank_penalty > 0.f) {
     sub_column_kernel<<<(int)((M + 255) / 256), 256, 0, stream>>>(logits, ldv, (int)M, blank_id, blank_penalty);
     RVB_COUNT_LAUNCH();
@@ -1126,7 +1042,7 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
                              const int* h_hyps, int L, const float* h_cat, int n_cat, int k, float* h_val, int* h_idx,
                              cudaStream_t stream, float* h_logp = nullptr /* (S, V) full rows, optional */) {
   const rvb_model_config& c = m->cfg;
-  RVB_REQUIRE(m->finalized && m->dec_l.present, "decoder_step_topk: model has no decoder");
+  RVB_REQUIRE(m->finalized && m->w.dec_l.present, "decoder_step_topk: model has no decoder");
   RVB_REQUIRE(L >= 1 && k >= 1 && k <= 16 && k <= c.vocab, "decoder_step_topk: bad L=%d / k=%d", L, k);
   const int S = B * N;
   const long long R = (long long)S * L, Mem = (long long)B * Tp;
@@ -1151,7 +1067,7 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   bf16* encbf;
   if (enc_operand(m, d_enc_out, Mem, &encbf, stream)) return -1;
   float* d_rows = h_logp ? m->ws_step_rows.as<float>() : nullptr;
-  if (decoder_pass(m, m->dec_l, encbf, dp + R + S, B, Tp, N, L, dp, dp + R, nullptr, nullptr, stream, k, d_val, d_idx,
+  if (decoder_pass(m, m->w.dec_l, encbf, dp + R + S, B, Tp, N, L, dp, dp + R, nullptr, nullptr, stream, k, d_val, d_idx,
                    d_rows))
     return -1;
   RVB_CHECK_CUDA(cudaMemcpyAsync(m->pin_c.p, d_val, out_bytes, cudaMemcpyDeviceToHost, stream));
@@ -1180,23 +1096,16 @@ struct DecCache {
   DecRows rows;  // S rows (kv unused: `cross` holds the source-attention keys / values)
   DevBuf logits, outv;
   HostPinned pin;
-  void release() {
-    for (auto* v : {&self_a, &self_b, &cross})
-      for (auto& b : *v) b.release();
-    for (DevBuf* b : {&ints, &logits, &outv}) b->release();
-    rows.release();
-    pin.release();
-  }
 };
 
 static int decoder_cache_begin(rvb_model* m, const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int N,
                                int Lcap, const float* h_cat, int n_cat, cudaStream_t stream) {
   const rvb_model_config& c = m->cfg;
-  RVB_REQUIRE(m->finalized && m->dec_l.present, "decoder_cache_begin: model has no decoder");
+  RVB_REQUIRE(m->finalized && m->w.dec_l.present, "decoder_cache_begin: model has no decoder");
   RVB_REQUIRE(B > 0 && Tp > 0 && N > 0 && Lcap > 0, "decoder_cache_begin: bad shape");
-  if (m->dcache == nullptr) m->dcache = new DecCache();
+  if (m->dcache == nullptr) m->dcache.reset(new DecCache());
   DecCache& dc = *m->dcache;
-  Decoder& D = m->dec_l;
+  Decoder& D = m->w.dec_l;
   const int d = c.d_model, S = B * N;
   const size_t pm = (size_t)m->pm(), nl = D.layers.size();
   const long long Mem = (long long)B * Tp;
@@ -1230,7 +1139,7 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
   const rvb_model_config& c = m->cfg;
   RVB_REQUIRE(m->dcache != nullptr && m->dcache->S > 0, "decoder_cache_step: call decoder_cache_begin first");
   DecCache& dc = *m->dcache;
-  Decoder& D = m->dec_l;
+  Decoder& D = m->w.dec_l;
   const int d = c.d_model, H = c.dec_heads, V = c.vocab, S = dc.S, B = dc.B, N = dc.N, pos = dc.step;
   RVB_REQUIRE(pos < dc.Lcap, "decoder_cache_step: step %d exceeds the cache capacity %d", pos, dc.Lcap);
   RVB_REQUIRE(k >= 1 && k <= 16 && k <= V, "decoder_cache_step: bad k=%d", k);
@@ -1407,8 +1316,8 @@ static int rescoring_flat(rvb_model* m, const NBest& nb, const float* d_enc_out,
     return -1;
   bf16* encbf;
   if (enc_operand(m, d_enc_out, (long long)nb.B * Tp, &encbf, stream)) return -1;
-  if (decoder_pass(m, m->dec_l, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
-  if (use_r && decoder_pass(m, m->dec_r, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_r, slen, gat_r, d_sc_r, stream))
+  if (decoder_pass(m, m->w.dec_l, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
+  if (use_r && decoder_pass(m, m->w.dec_r, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_r, slen, gat_r, d_sc_r, stream))
     return -1;
   return 0;
 }
@@ -1422,10 +1331,10 @@ static void unreverse_r2l(const NBest& nb, int Lp, float* r2l) {
 static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* h_enc_lens, int B, int Tp,
                                const int* h_tok, const int* h_len, int N, int max_len, const float* h_cat, int n_cat,
                                float reverse_weight, float* h_l2r, float* h_r2l, cudaStream_t stream) {
-  RVB_REQUIRE(m->finalized && m->dec_l.present, "attention_rescoring: model has no decoder");
+  RVB_REQUIRE(m->finalized && m->w.dec_l.present, "attention_rescoring: model has no decoder");
   const int Lp = max_len + 1, S = B * N;
   const long long R = (long long)S * Lp;
-  const bool use_r = reverse_weight > 0.f && m->dec_r.present && h_r2l != nullptr;
+  const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
   if (fold_lang(m, h_cat, n_cat, stream)) return -1;
   // the caller's hypotheses as an n-best with every slot present: an absent row (length < 0) is an empty hypothesis
   NBest& nb = m->nbest_in;
@@ -1497,14 +1406,9 @@ struct SearchTicket {
   int Lmax = 1;
   bool use_r = false;
   float* h_r2l = nullptr;
-  void release() {
-    nb.release();
-    trie.release();
-    nodes.release();
+  ~SearchTicket() {
     if (ev_search) cudaEventDestroy(ev_search);
     if (ev_done) cudaEventDestroy(ev_done);
-    ev_search = ev_done = nullptr;
-    state = 0;
   }
 };
 
@@ -1539,8 +1443,8 @@ static int search_submit(rvb_model* m, SearchTicket& t, const float* d_topk_val,
   t.d_enc_out = d_enc_out;
   // prefix trees of the n-best for the tree-structured rescoring decoder (left-to-right, and reversed when the model
   // has a right-to-left decoder): built right behind the search, their node counts travel with the lengths
-  t.has_trie = rescore_trie() && m->dec_l.present && beam <= 16;
-  t.has_rtrie = t.has_trie && m->dec_r.present;
+  t.has_trie = rescore_trie() && m->w.dec_l.present && beam <= 16;
+  t.has_rtrie = t.has_trie && m->w.dec_r.present;
   t.trie_stride = Tp + 1;
   t.trie_cap = beam * Tp + 1;
   const int ndir = t.has_trie ? (t.has_rtrie ? 2 : 1) : 0;
@@ -1612,11 +1516,11 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
   t.use_r = false;
   t.h_r2l = nullptr;
   if (run_decoder) {
-    RVB_REQUIRE(m->finalized && m->dec_l.present, "beam_search_rescoring: model has no decoder");
+    RVB_REQUIRE(m->finalized && m->w.dec_l.present, "beam_search_rescoring: model has no decoder");
     if (fold_lang(m, h_cat, n_cat, stream)) return -1;
     const int Lp = Lmax + 1;
     const long long R = (long long)S * Lp;
-    const bool use_r = reverse_weight > 0.f && m->dec_r.present && h_r2l != nullptr;
+    const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
     const size_t rints = (size_t)R * 4 + S;
     if (m->ws_misc.ensure(rints * sizeof(int) + (size_t)R * 2 * sizeof(float))) return -1;
     int* dp = m->ws_misc.as<int>();
@@ -1631,7 +1535,7 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
         int P = 1;
         for (int b = 0; b < B; ++b) P = hp_nodes[dir * B + b] > P ? hp_nodes[dir * B + b] : P;
         P = (P + 7) & ~7;
-        if (decoder_pass_trie(m, dir ? m->dec_r : m->dec_l, encbf, d.lens, B, Tp, N, Lp, P, t.trie_view(dir), d.olen,
+        if (decoder_pass_trie(m, dir ? m->w.dec_r : m->w.dec_l, encbf, d.lens, B, Tp, N, Lp, P, t.trie_view(dir), d.olen,
                               d.nhyp, dir ? d_sc_r : d_sc_l, stream))
           return -1;
       }
@@ -1664,12 +1568,24 @@ static int rescoring_collect(SearchTicket& t, int* h_lens, double* h_scores, int
 
 }  // namespace rvb
 
+// the buffers, the tickets and the decoder cache free themselves; a fork's weights belong to the parent's store
+rvb_model::~rvb_model() {
+  if (s_search) cudaStreamDestroy(s_search);
+  if (ev_topk) cudaEventDestroy(ev_topk);
+}
+
 // ================================================================================================================
 // C ABI
 extern "C" {
 
 RVB_API const char* rvb_last_error(void) { return rvb::last_error(); }
 RVB_API unsigned long long rvb_launch_count(void) { return rvb::g_launch_count.load(); }
+RVB_API int rvb_held_bytes(long long* device, long long* pinned) {
+  RVB_REQUIRE(device && pinned, "rvb_held_bytes: bad arguments");
+  *device = rvb::g_held_device.load();
+  *pinned = rvb::g_held_pinned.load();
+  return 0;
+}
 RVB_API int rvb_set_gemm_impl(int impl) {
   rvb::set_gemm_impl(impl);
   return 0;
@@ -1682,9 +1598,6 @@ RVB_API int rvb_gemm_profile_begin(void) {
 RVB_API int rvb_gemm_profile_end(double* total_ms, double* total_flops, long long* launches) {
   return rvb::gemm_profile_end(total_ms, total_flops, launches);
 }
-
-RVB_API void rvb_model_destroy(rvb_model* m);
-RVB_API int rvb_decoder_cache_end(rvb_model* m);
 
 RVB_API rvb_model* rvb_model_create(const rvb_model_config* cfg) {
   if (cfg == nullptr) {
@@ -1709,7 +1622,7 @@ RVB_API rvb_model* rvb_model_create(const rvb_model_config* cfg) {
 RVB_API int rvb_model_set_tensor(rvb_model* m, const char* name, const float* h_data, long long numel) {
   RVB_REQUIRE(m && name && h_data && numel >= 0, "rvb_model_set_tensor: bad arguments");
   RVB_REQUIRE(!m->finalized, "rvb_model_set_tensor: model already finalized");
-  m->host[name].assign(h_data, h_data + numel);
+  m->store.set(name, h_data, (size_t)numel);
   return 0;
 }
 
@@ -1731,36 +1644,16 @@ RVB_API rvb_model* rvb_model_fork(rvb_model* m) {
   f->cfg = m->cfg;
   f->x3 = m->x3;
   f->finalized = true;
-  f->cmvn_mean = m->cmvn_mean;
-  f->cmvn_istd = m->cmvn_istd;
-  f->conv1_w = m->conv1_w;
-  f->conv1_b = m->conv1_b;
-  f->conv2 = m->conv2;
-  f->embed = m->embed;
-  f->pos_all = m->pos_all;
-  f->enc = m->enc;
-  f->after_norm = m->after_norm;
-  f->ctc = m->ctc;
-  f->dec_l = m->dec_l;
-  f->dec_r = m->dec_r;
-  const int d = m->cfg.d_model;
-  auto own_fold = [&](rvb::Linear& L) -> int {
-    void* p = nullptr;
-    if (rvb::alloc_dev(f, (size_t)d * d * sizeof(rvb::bf16) * f->pm(), &p)) return -1;
-    L.w = reinterpret_cast<rvb::bf16*>(p);
-    if (rvb::alloc_dev(f, (size_t)d * sizeof(float), &p)) return -1;
-    L.b = reinterpret_cast<float*>(p);
-    return 0;
-  };
+  f->w = m->w;
   bool ok = true;
-  for (auto& E : f->enc)
-    if (E.lsl && own_fold(E.lang)) ok = false;
-  for (rvb::Decoder* D : {&f->dec_l, &f->dec_r})
+  for (auto& E : f->w.enc)
+    if (E.lsl && rvb::alloc_fold(f, &E.lang)) ok = false;
+  for (rvb::Decoder* D : {&f->w.dec_l, &f->w.dec_r})
     if (D->present)
       for (auto& Ld : D->layers)
-        if (Ld.lsl && own_fold(Ld.lang)) ok = false;
+        if (Ld.lsl && rvb::alloc_fold(f, &Ld.lang)) ok = false;
   if (!ok) {
-    rvb_model_destroy(f);
+    delete f;
     return nullptr;
   }
   return f;
@@ -1768,24 +1661,6 @@ RVB_API rvb_model* rvb_model_fork(rvb_model* m) {
 
 RVB_API void rvb_model_destroy(rvb_model* m) {
   if (!m) return;
-  for (void* p : m->owned) cudaFree(p);
-  DevBuf* bufs[] = {&m->ws_c1, &m->ws_c2, &m->ws_x, &m->ws_n, &m->ws_h, &m->ws_qkv, &m->ws_att, &m->ws_pw, &m->ws_cm,
-                    &m->ws_y, &m->ws_ybf, &m->ws_pe, &m->ws_pall, &m->ws_lens, &m->ws_encbf, &m->ws_logits,
-                    &m->ws_misc, &m->ws_kpp, &m->ws_cbias, &m->ws_fold, &m->ws_lse, &m->ws_tree_idx,
-                    &m->ws_edge_rows, &m->ws_edge_scores, &m->ws_step_rows, &m->ws_search};
-  for (DevBuf* b : bufs) b->release();
-  m->dec_rows.release();
-  m->nbest_in.release();
-  if (m->tickets) {
-    for (int i = 0; i < rvb_model::kTickets; ++i) m->tickets[i].release();
-    delete[] m->tickets;
-  }
-  rvb_decoder_cache_end(m);
-  if (m->s_search) cudaStreamDestroy(m->s_search);
-  if (m->ev_topk) cudaEventDestroy(m->ev_topk);
-  m->pin_a.release();
-  m->pin_b.release();
-  m->pin_c.release();
   delete m;
 }
 
@@ -1865,7 +1740,8 @@ RVB_API int rvb_logp_topk(const float* d_logp, int rows, int V, int k, float* d_
 }
 
 // per host thread: two decoding lanes (threads) may run the searches concurrently.  The model-less synchronous
-// searches only: the prefix beam search (workspace, n-best) and the greedy search (outputs, host copy).
+// searches only: the prefix beam search (workspace, n-best) and the greedy search (outputs, host copy).  Freed when
+// the thread exits.
 static thread_local rvb::DevBuf g_search_ws, g_search_out;
 static thread_local rvb::HostPinned g_search_pin;
 static thread_local rvb::NBest g_search_nb;
@@ -1944,7 +1820,7 @@ static int search_submit_any(rvb_model* m, const float* d_topk_val, const int* d
                              void* stream) {
   RVB_REQUIRE(m && d_topk_val && d_topk_idx && d_enc_out && h_enc_lens && B > 0 && Tp > 0 && beam > 0,
               "rvb_search_submit: bad arguments");
-  if (m->tickets == nullptr) m->tickets = new rvb::SearchTicket[rvb_model::kTickets];
+  if (m->tickets == nullptr) m->tickets.reset(new rvb::SearchTicket[rvb_model::kTickets]);
   int id = -1;
   for (int i = 0; i < rvb_model::kTickets; ++i)
     if (m->tickets[i].state == 0) {
@@ -2010,7 +1886,7 @@ RVB_API int rvb_beam_search_rescoring(rvb_model* m, const float* d_topk_val, con
   RVB_REQUIRE(m && d_topk_val && d_topk_idx && d_enc_out && h_enc_lens && h_tokens && h_times && h_lens && h_scores &&
                   h_nhyp && h_l2r && out_max_len && B > 0 && Tp > 0 && cap > 0,
               "rvb_beam_search_rescoring: bad arguments");
-  RVB_REQUIRE(m->finalized && m->dec_l.present, "beam_search_rescoring: model has no decoder");
+  RVB_REQUIRE(m->finalized && m->w.dec_l.present, "beam_search_rescoring: model has no decoder");
   const int id = rvb_search_submit(m, d_topk_val, d_topk_idx, k, d_enc_out, h_enc_lens, B, Tp, beam, blank_id, stream);
   if (id < 0) return -1;
   if (rvb_rescoring_submit(m, id, h_cat_embs, n_cat, reverse_weight, cap, 1, h_tokens, h_times, h_l2r, h_r2l, out_max_len,
@@ -2041,11 +1917,7 @@ RVB_API int rvb_decoder_cache_step(rvb_model* m, const int* h_tokens, const int*
 }
 
 RVB_API int rvb_decoder_cache_end(rvb_model* m) {
-  if (m && m->dcache) {
-    m->dcache->release();
-    delete m->dcache;
-    m->dcache = nullptr;
-  }
+  if (m) m->dcache.reset();
   return 0;
 }
 
