@@ -106,8 +106,12 @@ RVB_API int rvb_fbank_batch(const void* d_wave, int is_i16, int batch, long long
                             float* d_feats, long long n_frames, void* stream);
 
 /* feats (B, T, input_dim) fp32 -> enc_out (B, T', d_model) fp32; h_enc_lens[B] receives encoder_lens.
- * h_cat_embs: the LSL mixing weights [verbatimicity, 1 - verbatimicity] (n_cat == num_langs), may be NULL iff
- * num_langs == 0. */
+ * h_cat_embs: the LSL mixing weights [verbatimicity, 1 - verbatimicity], one vector (n_cat == num_langs) or one per
+ * utterance ((B, num_langs) row-major, n_cat == B * num_langs: utterance b decodes exactly as a batch whose every row
+ * carries row b); may be NULL iff num_langs == 0.  The same two lengths are accepted, with B the call's utterance count,
+ * by rvb_encoder_forward_chunked / _streaming, rvb_rescoring_submit, rvb_beam_search_rescoring,
+ * rvb_attention_rescoring, rvb_decoder_step_topk / _logp and rvb_decoder_cache_begin; in the decoder calls every
+ * hypothesis of utterance b uses row b.  Any other n_cat is an error. */
 RVB_API int rvb_encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat_lens, int B, int T,
                         const float* h_cat_embs, int n_cat, float* d_enc_out, int* h_enc_lens, void* stream);
 /* Same with bounded attention context — BaseEncoder.forward with decoding_chunk_size > 0 (encoder.py:117-149,
@@ -292,6 +296,14 @@ RVB_API int rvb_gemm_bf16_rows(const void* d_A, const void* d_W, const float* d_
  * (M, N) = (value half | residue half) of the N/2 GLU outputs; ldo = 0 selects that width. */
 RVB_API int rvb_gemm_bf16x3(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int act, int out_mode,
                             float alpha, void* d_out, int ldo, void* stream);
+/* The grouped GEMM of the language-specific layers with per-utterance mixing weights: d_W (N, K) and d_bias (N) stack
+ * N / group_n blocks of group_n rows (one folded linear per group).  Row m belongs to utterance m / rows_per_batch and is
+ * computed with the block of its group d_grp[m / rows_per_batch] (int32, device) only, into output columns
+ * [0, group_n) of d_out (ldo 0 -> group_n, or 2 * group_n for a bf16 pair).  Bit-equal to a plain rvb_gemm_bf16 /
+ * rvb_gemm_bf16x3 (x3 = 1) launch with that group's block.  out_mode 0 (bf16) or 1 (f32), no activation. */
+RVB_API int rvb_gemm_grouped(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int out_mode,
+                             void* d_out, int ldo, const int* d_grp, int rows_per_batch, int group_n, int x3,
+                             void* stream);
 /* (rows, width) fp32 -> (rows, 2 * width) bf16 = [hi | lo] */
 RVB_API int rvb_f32_to_bf16_pair(const float* d_x, void* d_out, long long rows, int width, void* stream);
 /* out[m] = log_softmax(A W^T + bias)[m, gather[m]] (0 where gather[m] < 0) without materialising the (M, N) logits:

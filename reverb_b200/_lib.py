@@ -91,6 +91,7 @@ SIGNATURES = {
     "rvb_gemm_bf16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _i, _vp]),
     "rvb_gemm_bf16_rows": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _i, _vp, _i, _vp]),
     "rvb_gemm_bf16x3": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _i, _vp]),
+    "rvb_gemm_grouped": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _i, _vp]),
     "rvb_f32_to_bf16_pair": (_i, [_vp, _vp, _ll, _i, _vp]),
     "rvb_gemm_logsoftmax_gather_ws_bytes": (_ll, [_i, _i]),
     "rvb_gemm_logsoftmax_gather": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),

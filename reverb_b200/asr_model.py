@@ -25,6 +25,13 @@ JOINT_DECODING_SOS = 10000        # hard-coded in the reference (transformer/sea
 JOINT_PRE_BEAM_RATIO = 1.5        # joint_decoding's default (search.py:457)
 
 
+def cat_row(cat_embs, b: int):
+    """Utterance b's mixing vector of a (num_langs,) or (B, num_langs) cat_embs."""
+    if cat_embs is None or torch.as_tensor(cat_embs).dim() < 2:
+        return cat_embs
+    return torch.as_tensor(cat_embs)[b]
+
+
 def alignment_result(a) -> DecodeResult:
     """engine.Alignment -> DecodeResult with `times` / `tokens_confidence` filled, so that it renders like a search
     result; the frame-level alignment travels as extra attributes."""
@@ -180,9 +187,9 @@ class ASRModel:
             mem = encoder_out[b:b + 1]
             mem_len = encoder_lens[b:b + 1]
 
-            def rows(prefixes, mem=mem, mem_len=mem_len):
+            def rows(prefixes, mem=mem, mem_len=mem_len, cat=cat_row(cat_embs, b)):
                 hy = np.asarray(prefixes, dtype=np.int32)
-                return self.engine.decoder_step_logp(mem, mem_len, hy, hy.shape[0], cat_embs)
+                return self.engine.decoder_step_logp(mem, mem_len, hy, hy.shape[0], cat)
             per_utt.append(time_sync_joint_search(val[b, :n], idx[b, :n], blank_lp[b, :n], rows, beam_size, ctc_weight,
                                                   length_bonus, JOINT_DECODING_SOS))
         return joint_decoding_results(per_utt)
@@ -216,6 +223,10 @@ class ASRModel:
                blank_id: int = 0, blank_penalty: float = 0.0, length_penalty: float = 0.0,
                infos: Optional[Dict[str, List[str]]] = None, cat_embs: Optional[torch.Tensor] = None,
                cv=None, cv_lengths=None) -> Dict[str, List[DecodeResult]]:
+        """The reference's decode(); cat_embs, the language-specific mixing weights [v, 1 - v] of verbatimicity v, is
+        (num_langs,) for the whole batch or (B, num_langs) with one row per utterance.  Row b decodes utterance b
+        exactly as a batch whose every row carries cat_embs[b], in all six modes; all hypotheses of utterance b use
+        cat_embs[b] (the reference's attention_rescoring / attention beam search at B = 1)."""
         st = self._stage_a(methods, speech, speech_lengths, beam_size, decoding_chunk_size, num_decoding_left_chunks,
                            ctc_weight, simulate_streaming, reverse_weight, context_graph, blank_id, blank_penalty,
                            length_penalty, infos, cat_embs, cv, cv_lengths)
@@ -227,7 +238,8 @@ class ASRModel:
     @torch.no_grad()
     def decode_stream(self, batches, methods: List[str], beam_size: int, **kwargs):
         """decode() over an iterable of (speech, speech_lengths) batches, software-pipelined on the current stream by
-        this one host thread; yields the per-batch result dicts in order.  Chunks are independent units
+        this one host thread; yields the per-batch result dicts in order.  A batch given as (speech, speech_lengths,
+        cat_embs) decodes with its own cat_embs instead of the keyword argument's.  Chunks are independent units
         (cli/reverb.py:214-234), so the results equal the batch-by-batch loop of the reference.
 
         Schedule (A = encoder + CTC head + prefix beam, B = decoder passes, C = collect + host score combination):
@@ -236,8 +248,9 @@ class ASRModel:
         the decoder batch) or combines the scores of batch n-2, the GPU still has a whole encoder pass queued."""
         inflight = []
         try:
-            for speech, speech_lengths in batches:
-                inflight.append(self._stage_a(methods, speech, speech_lengths, beam_size, **kwargs))
+            for batch in batches:
+                kw = kwargs if len(batch) == 2 else dict(kwargs, cat_embs=batch[2])
+                inflight.append(self._stage_a(methods, batch[0], batch[1], beam_size, **kw))
                 if len(inflight) >= 2:
                     self._stage_b(inflight[-2])
                 if len(inflight) >= 3:

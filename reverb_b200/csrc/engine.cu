@@ -74,6 +74,7 @@ struct EncLayer {
   float* bn_mean = nullptr;
   float* bn_var = nullptr;
   bool lsl = false;
+  int lsl_idx = -1;                    // index among the encoder's LSL layers (LangStack)
   std::vector<float*> lang_w, lang_b;  // fp32 device copies of language_layers.{i}
   Linear lang;                         // folded with the current cat_embs
 };
@@ -83,12 +84,37 @@ struct DecLayer {
   float eps = 1e-5f;
   Linear qkv, so, cq, ckv, co, ff1, ff2;
   bool lsl = false;
+  int lsl_idx = -1;  // index among the LSL layers of both decoders (LangStack)
   std::vector<float*> lang_w, lang_b;
   Linear lang;
 };
 
 struct SearchTicket;
 struct DecCache;
+
+// The folds of the G distinct mixing vectors of a per-utterance cat_embs, side by side for every LSL layer of the
+// encoder (or of the decoders): weight (G*d, d) — the (G*d, 2d) pair layout in the accurate mode — and bias (G*d),
+// grow-only, read by the grouped LSL GEMM (GemmArgs::grp).  `key` holds the vectors they were folded for, in group
+// order: a batch with the same ordered set folds nothing.
+struct LangStack {
+  std::vector<DevBuf> w, b;  // by lsl_idx
+  std::vector<float> key;
+};
+
+// The language-specific mixing of one call's utterances: uniform (G == 0: the layers' folded Linear), or G groups
+// with each utterance's group id on the device (owned by the call, its ticket or its decoder cache) and
+// rows_per_batch GEMM rows per utterance.
+struct CatRows {
+  int G = 0;
+  const int* d_grp = nullptr;
+  const LangStack* st = nullptr;
+  int rows_per_batch = 0;
+  CatRows rows(int rpb) const {
+    CatRows c = *this;
+    c.rows_per_batch = rpb;
+    return c;
+  }
+};
 
 struct Decoder {
   float* emb = nullptr;  // (V, d) fp32
@@ -177,6 +203,9 @@ struct rvb_model {
   bool finalized = false;
   Weights w;
   std::vector<float> cur_cat;  // cat_embs the LSL folds were computed for
+  rvb::LangStack st_enc, st_dec;  // stacked folds of per-utterance cat_embs (encoder, decoders)
+  DevBuf ws_grp;                  // group ids of attention_rescoring, which waits for its stream before it returns
+  HostPinned pin_grp;
   bool x3 = false;             // cfg.precision == 1: bf16x3 "fp32-accurate" mode (GemmArgs::x3, kernels.h)
   int pm() const { return x3 ? 2 : 1; }  // physical width multiplier of every bf16 operand ([hi | lo] pairs)
   DevBuf ws_fold;              // fp32 scratch of the accurate mode (LSL folds, positional table)
@@ -323,7 +352,7 @@ static int load_lang(rvb_model* m, const std::string& prefix, int d, int n_lang,
   return alloc_fold(m, folded);
 }
 
-static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Decoder* dec) {
+static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Decoder* dec, int* n_lsl) {
   const rvb_model_config& c = m->cfg;
   const int d = c.d_model, V = c.vocab;
   const std::string p = "decoder." + side;
@@ -349,6 +378,7 @@ static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Deco
     if (load_linear(m, q + ".feed_forward.w_1", c.dec_ffn_dim, d, &L.ff1)) return -1;
     if (load_linear(m, q + ".feed_forward.w_2", d, c.dec_ffn_dim, &L.ff2)) return -1;
     if (L.lsl && load_lang(m, q, d, c.num_langs, &L.lang_w, &L.lang_b, &L.lang)) return -1;
+    if (L.lsl) L.lsl_idx = (*n_lsl)++;
   }
   dec->present = true;
   return 0;
@@ -431,16 +461,18 @@ static int finalize_model(rvb_model* m) {
         return -1;
     }
     if (E.lsl && load_lang(m, p, d, c.num_langs, &E.lang_w, &E.lang_b, &E.lang)) return -1;
+    if (E.lsl) E.lsl_idx = i == 0 ? 0 : 1;
   }
   if (upload_w(m, posw.data(), (size_t)L * d, d, &m->w.pos_all.w)) return -1;
   m->w.pos_all.N = L * d;
   m->w.pos_all.K = d;
   if (load_linear(m, "ctc.ctc_lo", c.vocab, d, &m->w.ctc)) return -1;
+  int n_dec_lsl = 0;
   if (c.dec_blocks > 0 && m->store.find("decoder.left_decoder.embed.0.weight")) {
-    if (load_decoder(m, "left_decoder", c.dec_blocks, &m->w.dec_l)) return -1;
+    if (load_decoder(m, "left_decoder", c.dec_blocks, &m->w.dec_l, &n_dec_lsl)) return -1;
   }
   if (c.r_dec_blocks > 0 && m->store.find("decoder.right_decoder.embed.0.weight")) {
-    if (load_decoder(m, "right_decoder", c.r_dec_blocks, &m->w.dec_r)) return -1;
+    if (load_decoder(m, "right_decoder", c.r_dec_blocks, &m->w.dec_r, &n_dec_lsl)) return -1;
   }
   m->store.drop_host();
   m->finalized = true;
@@ -474,6 +506,92 @@ static int fold_lang(rvb_model* m, const float* cat, int n_cat, cudaStream_t str
   return 0;
 }
 
+// cat_embs of one call over B utterances: n_cat == num_langs (one vector) or B * num_langs (one per utterance).
+// -> the distinct vectors in order of first appearance (rows with equal bits are one vector), each utterance's group.
+static int group_cat(const rvb_model* m, const float* cat, int n_cat, int B, std::vector<float>* uniq,
+                     std::vector<int>* grp) {
+  const int L = m->cfg.num_langs;
+  uniq->clear();
+  grp->assign(B, 0);
+  if (L == 0) return 0;
+  RVB_REQUIRE(cat != nullptr && (n_cat == L || n_cat == B * L),
+              "cat_embs of length %d (one vector) or %d (one per utterance, B = %d) required (got %d)", L, B * L, B,
+              n_cat);
+  for (int b = 0; b < (n_cat == L ? 1 : B); ++b) {
+    const float* v = cat + (size_t)b * L;
+    const int G = (int)uniq->size() / L;
+    int g = 0;
+    while (g < G && memcmp(uniq->data() + (size_t)g * L, v, sizeof(float) * L) != 0) ++g;
+    if (g == G) uniq->insert(uniq->end(), v, v + L);
+    (*grp)[b] = g;
+  }
+  return 0;
+}
+
+// fold each of the G vectors of `cat` (G * num_langs) the way fold_lang folds one, into the stacked folds of the
+// encoder's (dec = false) or the decoders' LSL layers, on the stream of the kernels that read them
+static int fold_stack(rvb_model* m, bool dec, const std::vector<float>& cat, cudaStream_t stream) {
+  LangStack& st = dec ? m->st_dec : m->st_enc;
+  if (st.key.size() == cat.size() && memcmp(st.key.data(), cat.data(), sizeof(float) * cat.size()) == 0) return 0;
+  st.key.clear();
+  const int d = m->cfg.d_model, L = m->cfg.num_langs, G = (int)cat.size() / L;
+  const size_t pm = (size_t)m->pm();
+  if (m->x3 && m->ws_fold.ensure((size_t)d * d * sizeof(float))) return -1;
+  auto fold = [&](std::vector<float*>& lw, std::vector<float*>& lb, int idx) -> int {
+    if ((int)st.w.size() <= idx) {
+      st.w.resize(idx + 1);
+      st.b.resize(idx + 1);
+    }
+    if (st.w[idx].ensure((size_t)G * d * d * pm * sizeof(bf16)) || st.b[idx].ensure((size_t)G * d * sizeof(float)))
+      return -1;
+    for (int g = 0; g < G; ++g) {
+      const float* c = cat.data() + (size_t)g * L;
+      bf16* w = st.w[idx].as<bf16>() + (size_t)g * d * d * pm;
+      if (m->x3) {
+        float* tmp = m->ws_fold.as<float>();
+        if (launch_weighted_sum_bf16(lw.data(), c, L, (long long)d * d, nullptr, tmp, stream)) return -1;
+        if (launch_f32_to_pair(tmp, w, d, d, stream)) return -1;
+      } else if (launch_weighted_sum_bf16(lw.data(), c, L, (long long)d * d, w, nullptr, stream)) return -1;
+      if (launch_weighted_sum_bf16(lb.data(), c, L, d, nullptr, st.b[idx].as<float>() + (size_t)g * d, stream)) return -1;
+    }
+    return 0;
+  };
+  if (!dec) {
+    for (auto& E : m->w.enc)
+      if (E.lsl && fold(E.lang_w, E.lang_b, E.lsl_idx)) return -1;
+  } else {
+    for (Decoder* D : {&m->w.dec_l, &m->w.dec_r})
+      if (D->present)
+        for (auto& Ld : D->layers)
+          if (Ld.lsl && fold(Ld.lang_w, Ld.lang_b, Ld.lsl_idx)) return -1;
+  }
+  st.key = cat;
+  return 0;
+}
+
+// The one place that chooses between the uniform and the grouped LSL path of a call: one distinct vector (cat_embs of
+// num_langs, or B rows with equal bits) runs fold_lang and the plain launches; G > 1 distinct vectors fold the stack of
+// the encoder (dec = false) or of the decoders.  -> *G (0 = uniform), uniq (the vectors), grp (each utterance's group).
+static int prepare_cat(rvb_model* m, bool dec, const float* cat, int n_cat, int B, std::vector<float>* uniq,
+                       std::vector<int>* grp, int* G, cudaStream_t stream) {
+  if (group_cat(m, cat, n_cat, B, uniq, grp)) return -1;
+  const int L = m->cfg.num_langs;
+  *G = L ? (int)uniq->size() / L : 0;
+  if (*G <= 1) {
+    *G = 0;
+    return L ? fold_lang(m, uniq->data(), L, stream) : 0;
+  }
+  return fold_stack(m, dec, *uniq, stream);
+}
+
+// B group ids -> dev through the page-locked pin, on `stream`
+static int upload_groups(const std::vector<int>& grp, HostPinned& pin, DevBuf& dev, cudaStream_t stream) {
+  if (pin.ensure(grp.size() * sizeof(int)) || dev.ensure(grp.size() * sizeof(int))) return -1;
+  memcpy(pin.p, grp.data(), grp.size() * sizeof(int));
+  RVB_CHECK_CUDA(cudaMemcpyAsync(dev.p, pin.p, grp.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  return 0;
+}
+
 // <sos>/<eos>: tokenizer_conf.special_tokens when the config names them, else vocab - 1 for both (asr_model.py:79-82)
 static inline int sos_id(const rvb_model_config& c) { return c.sos_id > 0 ? c.sos_id : c.vocab - 1; }
 static inline int eos_id(const rvb_model_config& c) { return c.eos_id > 0 ? c.eos_id : c.vocab - 1; }
@@ -497,6 +615,30 @@ static int gemm(rvb_model* m, const bf16* A, const Linear& W, int M, int act, in
   g.row_lens = row_lens;
   g.rows_per_batch = rows_per_batch;
   g.ldo = ldo;
+  return launch_gemm(g, stream);
+}
+
+// The language-specific linear of one LSL layer over M rows: the uniformly folded weight `uni`, or one grouped launch
+// over the stacked folds (layer lsl_idx of cr.st), every row taking its utterance's fold
+static int lang_gemm(rvb_model* m, const bf16* A, const Linear& uni, int lsl_idx, const CatRows& cr, int M, int out_mode,
+                     void* out, cudaStream_t stream) {
+  if (cr.G == 0) return gemm(m, A, uni, M, ACT_NONE, out_mode, out, 1.f, stream);
+  const int d = m->cfg.d_model;
+  GemmArgs g;
+  g.x3 = m->x3 ? 1 : 0;
+  if (m->x3 && out_mode == OUT_BF16) g.out_split = d;
+  g.A = A;
+  g.W = cr.st->w[lsl_idx].as<bf16>();
+  g.M = M;
+  g.N = cr.G * d;
+  g.K = d;
+  g.bias = cr.st->b[lsl_idx].as<float>();
+  g.act = ACT_NONE;
+  g.out_mode = out_mode;
+  g.out = out;
+  g.grp = cr.d_grp;
+  g.group_n = d;
+  g.rows_per_batch = cr.rows_per_batch;
   return launch_gemm(g, stream);
 }
 
@@ -606,26 +748,35 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
   const int T1h = (T1 + 1) / 2;
   const long long M = (long long)B * Tp;
   RVB_REQUIRE(M * (long long)F2 < (1ll << 31), "encoder_forward: batch too large (B*T'*F2 overflows int)");
-  if (fold_lang(m, h_cat, n_cat, stream)) return -1;
+  std::vector<float> cat_u;
+  std::vector<int> grp;
+  CatRows cr;
+  if (prepare_cat(m, false, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
 
   // lengths
   // pinned staging ring: a back-to-back call must not overwrite lengths an earlier async copy still reads.  Slots are
   // sized for the largest batch seen, so batches of varying B (corpus decoding) only wait when that maximum grows.
+  // A slot holds the lengths (lens_cap) and then the utterances' LSL groups of a per-utterance cat_embs.
   constexpr int kRing = 16;
   if (B > m->lens_cap) {
     RVB_CHECK_CUDA(cudaStreamSynchronize(stream));
-    if (m->pin_a.ensure(sizeof(int) * B * kRing) || m->ws_lens.ensure(sizeof(int) * B * kRing)) return -1;
+    if (m->pin_a.ensure(sizeof(int) * 2 * B * kRing) || m->ws_lens.ensure(sizeof(int) * 2 * B * kRing)) return -1;
     m->lens_cap = B;
   }
   const int slot = (m->lens_slot++) % kRing;
-  int* h_lens = m->pin_a.as<int>() + (size_t)slot * m->lens_cap;
+  int* h_lens = m->pin_a.as<int>() + (size_t)slot * 2 * m->lens_cap;
   for (int b = 0; b < B; ++b) {
     int e = rvb_encoder_out_len(h_feat_lens[b], T);
     h_lens[b] = e;
     if (h_enc_lens) h_enc_lens[b] = e;
   }
-  int* d_lens = m->ws_lens.as<int>() + (size_t)slot * m->lens_cap;
-  RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, h_lens, sizeof(int) * B, cudaMemcpyHostToDevice, stream));
+  int* d_lens = m->ws_lens.as<int>() + (size_t)slot * 2 * m->lens_cap;
+  if (cr.G) memcpy(h_lens + m->lens_cap, grp.data(), sizeof(int) * B);
+  RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, h_lens, sizeof(int) * (cr.G ? m->lens_cap + B : B), cudaMemcpyHostToDevice,
+                                 stream));
+  cr.d_grp = d_lens + m->lens_cap;
+  cr.st = &m->st_enc;
+  cr.rows_per_batch = Tp;
 
   // workspace
   const bool x3 = m->x3;
@@ -840,7 +991,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     if (launch_layernorm(x, E.norm_ff.g, E.norm_ff.b, 1e-5f, (int)M, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
     const bf16* ffn_in = n;
     if (E.lsl) {
-      if (gemm(m, n, E.lang, (int)M, ACT_NONE, OUT_F32, y, 1.f, stream)) return -1;
+      if (lang_gemm(m, n, E.lang, E.lsl_idx, cr, (int)M, OUT_F32, y, stream)) return -1;
       if (x3 ? launch_f32_to_pair(y, ybf, M, d, stream) : launch_f32_to_bf16(y, ybf, M * d, stream)) return -1;
       ffn_in = ybf;
     }
@@ -891,9 +1042,10 @@ static int ctc_topk(rvb_model* m, const float* d_enc_out, int B, int Tp, int k, 
 // The layers of a (LanguageSpecific)TransformerDecoder over the R rows of w.x, then after_norm -> w.n
 // (decoder_layer.py:95-110 / 286-301).  self_attn(l) attends from the [q | k | v] projection in w.qkv, src_attn(l) from
 // the q projection in w.qkv (row stride d) over the encoder output; both write w.att.
+// cr: the LSL mixing of the rows' utterances (cr.rows_per_batch rows each).
 template <class SelfAttn, class SrcAttn>
-static int decoder_layers(rvb_model* m, Decoder& D, DecRows& w, int R, SelfAttn self_attn, SrcAttn src_attn,
-                          cudaStream_t stream) {
+static int decoder_layers(rvb_model* m, Decoder& D, DecRows& w, int R, const CatRows& cr, SelfAttn self_attn,
+                          SrcAttn src_attn, cudaStream_t stream) {
   const int d = m->cfg.d_model;
   const bool x3 = m->x3;
   float* x = w.x.as<float>();
@@ -918,7 +1070,7 @@ static int decoder_layers(rvb_model* m, Decoder& D, DecRows& w, int R, SelfAttn 
     if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
     const bf16* ffn_in = n;
     if (Ld.lsl) {
-      if (gemm(m, n, Ld.lang, R, ACT_NONE, OUT_BF16, ybf, 1.f, stream)) return -1;
+      if (lang_gemm(m, n, Ld.lang, Ld.lsl_idx, cr, R, OUT_BF16, ybf, stream)) return -1;
       ffn_in = ybf;
     }
     if (gemm(m, ffn_in, Ld.ff1, R, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
@@ -991,7 +1143,7 @@ static int last_position_topk(rvb_model* m, const Decoder& D, const bf16* n, int
 // layer; log_softmax + top-step_k of it -> d_step_val / d_step_idx (S, step_k).
 static int decoder_pass(rvb_model* m, Decoder& D, const bf16* enc_bf, const int* d_enc_lens, int B, int Tp, int N,
                         int Lp, const int* d_tokens, const int* d_seq_lens, const int* d_gather, float* d_scores,
-                        cudaStream_t stream, int step_k = 0, float* d_step_val = nullptr, int* d_step_idx = nullptr,
+                        const CatRows& cr, cudaStream_t stream, int step_k = 0, float* d_step_val = nullptr, int* d_step_idx = nullptr,
                         float* d_step_logp = nullptr /* (S, V): full log_softmax rows of the last position */) {
   const rvb_model_config& c = m->cfg;
   const int d = c.d_model, H = c.dec_heads, dk = d / H, V = c.vocab;
@@ -1028,7 +1180,7 @@ static int decoder_pass(rvb_model* m, Decoder& D, const bf16* enc_bf, const int*
     if (gemm(m, enc_bf, D.layers[l].ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
     return dec_attention(m, src_attention(qkv, kv, att, d, B, N * Lp, Tp, H, d_enc_lens), stream);
   };
-  if (decoder_layers(m, D, w, (int)R, self_attn, src_attn, stream)) return -1;
+  if (decoder_layers(m, D, w, (int)R, cr.rows(N * Lp), self_attn, src_attn, stream)) return -1;
   if (step_k > 0)
     return last_position_topk(m, D, w.n.as<bf16>(), S, Lp, m->ws_logits, step_k, d_step_val, d_step_idx, d_step_logp,
                               stream);
@@ -1046,8 +1198,11 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   RVB_REQUIRE(L >= 1 && k >= 1 && k <= 16 && k <= c.vocab, "decoder_step_topk: bad L=%d / k=%d", L, k);
   const int S = B * N;
   const long long R = (long long)S * L, Mem = (long long)B * Tp;
-  if (fold_lang(m, h_cat, n_cat, stream)) return -1;
-  const size_t ints = (size_t)R + S + B;
+  std::vector<float> cat_u;
+  std::vector<int> grp;
+  CatRows cr;
+  if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+  const size_t ints = (size_t)R + S + 2 * B;   // tokens | lengths | encoder lengths | LSL groups
   const size_t out_bytes = (size_t)S * k * (sizeof(float) + sizeof(int));
   const size_t row_bytes = h_logp ? (size_t)S * c.vocab * sizeof(float) : 0;
   if (m->pin_b.ensure(ints * sizeof(int)) || m->ws_misc.ensure(ints * sizeof(int) + out_bytes) ||
@@ -1060,15 +1215,18 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   }
   for (int s = 0; s < S; ++s) hp[R + s] = L;
   for (int b = 0; b < B; ++b) hp[R + S + b] = h_enc_lens[b];
+  for (int b = 0; b < B; ++b) hp[R + S + B + b] = grp[b];
   int* dp = m->ws_misc.as<int>();
+  cr.d_grp = dp + R + S + B;
+  cr.st = &m->st_dec;
   RVB_CHECK_CUDA(cudaMemcpyAsync(dp, hp, ints * sizeof(int), cudaMemcpyHostToDevice, stream));
   float* d_val = reinterpret_cast<float*>(dp + ints);
   int* d_idx = reinterpret_cast<int*>(d_val + (size_t)S * k);
   bf16* encbf;
   if (enc_operand(m, d_enc_out, Mem, &encbf, stream)) return -1;
   float* d_rows = h_logp ? m->ws_step_rows.as<float>() : nullptr;
-  if (decoder_pass(m, m->w.dec_l, encbf, dp + R + S, B, Tp, N, L, dp, dp + R, nullptr, nullptr, stream, k, d_val, d_idx,
-                   d_rows))
+  if (decoder_pass(m, m->w.dec_l, encbf, dp + R + S, B, Tp, N, L, dp, dp + R, nullptr, nullptr, cr, stream, k, d_val,
+                   d_idx, d_rows))
     return -1;
   RVB_CHECK_CUDA(cudaMemcpyAsync(m->pin_c.p, d_val, out_bytes, cudaMemcpyDeviceToHost, stream));
   if (h_logp)
@@ -1096,6 +1254,10 @@ struct DecCache {
   DecRows rows;  // S rows (kv unused: `cross` holds the source-attention keys / values)
   DevBuf logits, outv;
   HostPinned pin;
+  std::vector<float> cat;  // the distinct LSL mixing vectors of decoder_cache_begin, refolded (if need be) every step
+  int G = 0;               // CatRows::G of the cached utterances, their groups in grp
+  DevBuf grp;
+  HostPinned grp_pin;
 };
 
 static int decoder_cache_begin(rvb_model* m, const float* d_enc_out, const int* h_enc_lens, int B, int Tp, int N,
@@ -1109,7 +1271,9 @@ static int decoder_cache_begin(rvb_model* m, const float* d_enc_out, const int* 
   const int d = c.d_model, S = B * N;
   const size_t pm = (size_t)m->pm(), nl = D.layers.size();
   const long long Mem = (long long)B * Tp;
-  if (fold_lang(m, h_cat, n_cat, stream)) return -1;
+  std::vector<int> grp;
+  if (prepare_cat(m, true, h_cat, n_cat, B, &dc.cat, &grp, &dc.G, stream)) return -1;
+  if (dc.G && upload_groups(grp, dc.grp_pin, dc.grp, stream)) return -1;
   dc.B = B; dc.Tp = Tp; dc.N = N; dc.S = S; dc.Lcap = Lcap; dc.step = 0; dc.flip = false;
   dc.self_a.resize(nl); dc.self_b.resize(nl); dc.cross.resize(nl);
   const size_t kvw = (size_t)2 * d * pm;  // cache row: [k | v] (x2 for the hi / lo pair layout)
@@ -1162,6 +1326,13 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
   std::vector<DevBuf>& cur = dc.flip ? dc.self_b : dc.self_a;
   std::vector<DevBuf>& nxt = dc.flip ? dc.self_a : dc.self_b;
   const bool reorder = h_parents != nullptr && pos > 0;
+  CatRows cr;   // the folds of decoder_cache_begin's vectors: a call in between may have folded others
+  cr.G = dc.G;
+  cr.d_grp = dc.grp.as<int>();
+  cr.st = &m->st_dec;
+  cr.rows_per_batch = N;
+  if (c.num_langs && (dc.G ? fold_stack(m, true, dc.cat, stream) : fold_lang(m, dc.cat.data(), c.num_langs, stream)))
+    return -1;
   bf16* qkv = dc.rows.qkv.as<bf16>();
   bf16* att = dc.rows.att.as<bf16>();
   if (launch_embed_posenc(d_tok, D.emb, S, 1, d, dc.rows.x.as<float>(), stream, pos)) return -1;
@@ -1196,7 +1367,7 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
     a.f32 = true;
     return dec_attention(m, a, stream);
   };
-  if (decoder_layers(m, D, dc.rows, S, self_attn, src_attn, stream)) return -1;
+  if (decoder_layers(m, D, dc.rows, S, cr, self_attn, src_attn, stream)) return -1;
   if (reorder) dc.flip = !dc.flip;
   float* d_val = dc.outv.as<float>();
   int* d_idx = reinterpret_cast<int*>(d_val + (size_t)S * k);
@@ -1232,7 +1403,7 @@ struct TrieView {
 
 static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const int* d_enc_lens, int B, int Tp, int N,
                              int Lp, int P, const TrieView& tv, const int* d_olen, const int* d_nhyp, float* d_scores,
-                             cudaStream_t stream) {
+                             const CatRows& cr, cudaStream_t stream) {
   const rvb_model_config& c = m->cfg;
   const int d = c.d_model, H = c.dec_heads, dk = d / H;
   const long long R = (long long)B * P, E = (long long)B * (P + N), Mem = (long long)B * Tp;
@@ -1295,7 +1466,7 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
     if (gemm(m, enc_bf, D.layers[l].ckv, (int)Mem, ACT_NONE, OUT_BF16, kv, 1.f, stream)) return -1;
     return dec_attention(m, src_attention(qkv, kv, att, d, B, P, Tp, H, d_enc_lens), stream);
   };
-  if (decoder_layers(m, D, w, (int)R, self_attn, src_attn, stream)) return -1;
+  if (decoder_layers(m, D, w, (int)R, cr.rows(P), self_attn, src_attn, stream)) return -1;
   // output layer on one row per EDGE of the tree (+ one per hypothesis end): hidden state of the edge's source node
   if (launch_gather_rows(w.n.as<bf16>(), src, a_out, (int)E, d * (int)pm, stream)) return -1;
   if (target_logp(m, D, a_out, (int)E, tgt, e_sc, stream)) return -1;
@@ -1307,7 +1478,7 @@ static int decoder_pass_trie(rvb_model* m, Decoder& D, const bf16* enc_bf, const
 // [sos, w_1..w_U, eos..] and the reversed variant (asr_model.py:921-949), the gather targets gat_l / gat_r (-1 = none,
 // search.py:417-430) and slen = U + 1; absent hypotheses are empty.  -> d_sc_l / d_sc_r (R) log-probs of the targets.
 static int rescoring_flat(rvb_model* m, const NBest& nb, const float* d_enc_out, int Tp, int Lp, bool use_r, int* idx,
-                          float* d_sc_l, float* d_sc_r, cudaStream_t stream) {
+                          float* d_sc_l, float* d_sc_r, const CatRows& cr, cudaStream_t stream) {
   const NBest::Arrays d = nb.d();
   const size_t R = nb.S() * Lp;
   int *tok_l = idx, *tok_r = idx + R, *gat_l = idx + 2 * R, *gat_r = idx + 3 * R, *slen = idx + 4 * R;
@@ -1316,8 +1487,8 @@ static int rescoring_flat(rvb_model* m, const NBest& nb, const float* d_enc_out,
     return -1;
   bf16* encbf;
   if (enc_operand(m, d_enc_out, (long long)nb.B * Tp, &encbf, stream)) return -1;
-  if (decoder_pass(m, m->w.dec_l, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_l, slen, gat_l, d_sc_l, stream)) return -1;
-  if (use_r && decoder_pass(m, m->w.dec_r, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_r, slen, gat_r, d_sc_r, stream))
+  if (decoder_pass(m, m->w.dec_l, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_l, slen, gat_l, d_sc_l, cr, stream)) return -1;
+  if (use_r && decoder_pass(m, m->w.dec_r, encbf, d.lens, nb.B, Tp, nb.beam, Lp, tok_r, slen, gat_r, d_sc_r, cr, stream))
     return -1;
   return 0;
 }
@@ -1335,7 +1506,13 @@ static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* 
   const int Lp = max_len + 1, S = B * N;
   const long long R = (long long)S * Lp;
   const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
-  if (fold_lang(m, h_cat, n_cat, stream)) return -1;
+  std::vector<float> cat_u;
+  std::vector<int> grp;
+  CatRows cr;
+  if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+  if (cr.G && upload_groups(grp, m->pin_grp, m->ws_grp, stream)) return -1;
+  cr.d_grp = m->ws_grp.as<int>();
+  cr.st = &m->st_dec;
   // the caller's hypotheses as an n-best with every slot present: an absent row (length < 0) is an empty hypothesis
   NBest& nb = m->nbest_in;
   const size_t rints = (size_t)R * 4 + S;
@@ -1356,7 +1533,7 @@ static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* 
   int* idx = m->ws_misc.as<int>();
   float* d_sc_l = reinterpret_cast<float*>(idx + rints);
   float* d_sc_r = d_sc_l + R;
-  if (rescoring_flat(m, nb, d_enc_out, Tp, Lp, use_r, idx, d_sc_l, d_sc_r, stream)) return -1;
+  if (rescoring_flat(m, nb, d_enc_out, Tp, Lp, use_r, idx, d_sc_l, d_sc_r, cr, stream)) return -1;
   float* hs = m->pin_c.as<float>();
   RVB_CHECK_CUDA(cudaMemcpyAsync(hs, d_sc_l, (size_t)R * (use_r ? 2 : 1) * sizeof(float), cudaMemcpyDeviceToHost,
                                  stream));
@@ -1406,6 +1583,8 @@ struct SearchTicket {
   int Lmax = 1;
   bool use_r = false;
   float* h_r2l = nullptr;
+  DevBuf grp;          // LSL groups of the batch's utterances (per-utterance cat_embs)
+  HostPinned grp_pin;
   ~SearchTicket() {
     if (ev_search) cudaEventDestroy(ev_search);
     if (ev_done) cudaEventDestroy(ev_done);
@@ -1517,7 +1696,13 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
   t.h_r2l = nullptr;
   if (run_decoder) {
     RVB_REQUIRE(m->finalized && m->w.dec_l.present, "beam_search_rescoring: model has no decoder");
-    if (fold_lang(m, h_cat, n_cat, stream)) return -1;
+    std::vector<float> cat_u;
+    std::vector<int> grp;
+    CatRows cr;
+    if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+    if (cr.G && upload_groups(grp, t.grp_pin, t.grp, stream)) return -1;
+    cr.d_grp = t.grp.as<int>();
+    cr.st = &m->st_dec;
     const int Lp = Lmax + 1;
     const long long R = (long long)S * Lp;
     const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
@@ -1536,10 +1721,10 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
         for (int b = 0; b < B; ++b) P = hp_nodes[dir * B + b] > P ? hp_nodes[dir * B + b] : P;
         P = (P + 7) & ~7;
         if (decoder_pass_trie(m, dir ? m->w.dec_r : m->w.dec_l, encbf, d.lens, B, Tp, N, Lp, P, t.trie_view(dir), d.olen,
-                              d.nhyp, dir ? d_sc_r : d_sc_l, stream))
+                              d.nhyp, dir ? d_sc_r : d_sc_l, cr, stream))
           return -1;
       }
-    } else if (rescoring_flat(m, t.nb, t.d_enc_out, Tp, Lp, use_r, dp, d_sc_l, d_sc_r, stream)) {
+    } else if (rescoring_flat(m, t.nb, t.d_enc_out, Tp, Lp, use_r, dp, d_sc_l, d_sc_r, cr, stream)) {
       return -1;
     }
     RVB_CHECK_CUDA(cudaMemcpyAsync(h_l2r, d_sc_l, (size_t)R * sizeof(float), cudaMemcpyDeviceToHost, stream));
@@ -1995,6 +2180,28 @@ RVB_API int rvb_gemm_bf16x3(const void* d_A, const void* d_W, const float* d_bia
   g.ldo = ldo;
   g.x3 = 1;
   if (out_mode == rvb::OUT_BF16) g.out_split = (act == rvb::ACT_GLU) ? N / 2 : N;
+  return rvb::launch_gemm(g, (cudaStream_t)stream);
+}
+
+RVB_API int rvb_gemm_grouped(const void* d_A, const void* d_W, const float* d_bias, int M, int N, int K, int out_mode,
+                             void* d_out, int ldo, const int* d_grp, int rows_per_batch, int group_n, int x3,
+                             void* stream) {
+  rvb::GemmArgs g;
+  g.A = reinterpret_cast<const rvb::bf16*>(d_A);
+  g.W = reinterpret_cast<const rvb::bf16*>(d_W);
+  g.M = M;
+  g.N = N;
+  g.K = K;
+  g.bias = d_bias;
+  g.out_mode = out_mode;
+  g.out = d_out;
+  g.ldo = ldo;
+  g.grp = d_grp;
+  g.group_n = group_n;
+  g.rows_per_batch = rows_per_batch;
+  g.x3 = x3 ? 1 : 0;
+  if (x3 && out_mode == rvb::OUT_BF16) g.out_split = group_n;
+  RVB_REQUIRE(d_grp != nullptr, "rvb_gemm_grouped: null group array");
   return rvb::launch_gemm(g, (cudaStream_t)stream);
 }
 

@@ -23,6 +23,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <mutex>
 #include <vector>
 
@@ -72,6 +73,9 @@ struct GemmKParams {
   int glu_coalesced;   // ACT_GLU with 16-byte aligned output rows (always true after the launch checks)
   int bf16_coalesced;  // bf16 output rows are 16-byte aligned -> staged, coalesced epilogue (see drain_tile)
   int f32_coalesced;  // fp32 output rows are 16-byte aligned -> staged, coalesced epilogue (see drain_tile)
+  const int* grp;      // grouped output (GemmArgs::grp): group of each utterance of rows_per_batch rows, or nullptr
+  int group_n;         // output columns per group
+  int grp_slots;       // grouped output: utterance slots per M tile (the most utterances 128 rows can touch)
   // simt fallback only
   const bf16* A;
   const bf16* W;
@@ -80,16 +84,25 @@ struct GemmKParams {
 };
 
 struct TileCoord {
-  int n0;        // first output column
+  int n0;        // first accumulator column (of W / bias)
   int row0;      // plain: first row; conv: t0
   int b, f;      // conv only
+  int g;         // grouped output: the group of the tile's N block (0 otherwise); output column = n - g * group_n
 };
 
+// Grouped output: the tiles of M tile mt are (slot u, column block j) — u-th utterance among the tile's rows, j-th BN
+// block of that utterance's group — so a launch enumerates grp_slots * group_n / BN tiles per M tile, whatever G is.
 __device__ __forceinline__ TileCoord decode_tile(const GemmKParams& p, int tile, int BN) {
   TileCoord t;
   int nb = tile % p.tiles_n;
   int mt = tile / p.tiles_n;
   t.n0 = nb * BN;
+  t.g = 0;
+  if (p.grp != nullptr) {
+    const int nbg = p.group_n / BN;
+    t.g = __ldg(p.grp + (mt * 128) / p.rows_per_batch + nb / nbg);
+    t.n0 = t.g * p.group_n + (nb % nbg) * BN;
+  }
   if (p.conv_mode) {
     t.f = mt % p.conv_F2;
     int r = mt / p.conv_F2;
@@ -101,6 +114,22 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmKParams& p, int tile,
     t.f = 0;
   }
   return t;
+}
+
+// Whether a tile has rows to write: always, except under a grouped output, where its slot must hold an utterance of
+// the tile's rows whose group no earlier slot of the tile has (each group present among the rows is computed once).
+// The producer and both consumer warpgroups walk the CTA's tiles through this same predicate, so they agree on the
+// ring order.
+__device__ __forceinline__ bool tile_active(const GemmKParams& p, int tile, int BN) {
+  if (p.grp == nullptr) return true;
+  const int r0 = (tile / p.tiles_n) * 128;
+  const int b0 = r0 / p.rows_per_batch;
+  const int b = b0 + (tile % p.tiles_n) / (p.group_n / BN);
+  if (b > (min(r0 + 128, p.M) - 1) / p.rows_per_batch) return false;
+  const int g = __ldg(p.grp + b);
+  for (int e = b0; e < b; ++e)
+    if (__ldg(p.grp + e) == g) return false;
+  return true;
 }
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -145,7 +174,8 @@ __device__ __forceinline__ float2 gated2(float2 x, float2 g) {
 
 // One thread stores 32 consecutive output columns [n0, n0+32) of one output row (n0 % 32 == 0).
 template <int EPI>
-__device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_row, int n0, const uint32_t* acc) {
+// n0: accumulator (bias) column; the output column is n0 - oshift (grouped output: the group's first column)
+__device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_row, int n0, int oshift, const uint32_t* acc) {
   float v[32];
   const bool full = (n0 + 32 <= p.N);
   constexpr int OUT = (EPI <= EPI_BF16_SILU) ? OUT_BF16 : (EPI == EPI_F32) ? OUT_F32 : OUT_RESID_F32;
@@ -185,7 +215,7 @@ __device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_
     }
   }
   if (out_mode == OUT_BF16) {
-    bf16* o = reinterpret_cast<bf16*>(p.out) + out_row * p.ldo + n0;
+    bf16* o = reinterpret_cast<bf16*>(p.out) + out_row * p.ldo + n0 - oshift;
     if (full && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -201,7 +231,7 @@ __device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_
         if (n0 + j < p.N) o[j] = __float2bfloat16(v[j]);
     }
   } else if (out_mode == OUT_F32) {
-    float* o = reinterpret_cast<float*>(p.out) + out_row * p.ldo + n0;
+    float* o = reinterpret_cast<float*>(p.out) + out_row * p.ldo + n0 - oshift;
     if (full && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
 #pragma unroll
       for (int j = 0; j < 8; ++j)
@@ -211,7 +241,7 @@ __device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_
         if (n0 + j < p.N) o[j] = v[j];
     }
   } else {  // OUT_RESID_F32
-    float* o = reinterpret_cast<float*>(p.out) + out_row * p.ldo + n0;
+    float* o = reinterpret_cast<float*>(p.out) + out_row * p.ldo + n0 - oshift;
     if (full && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
       float4 r[8];
 #pragma unroll
@@ -275,6 +305,7 @@ __device__ __forceinline__ long long output_row(const GemmKParams& p, const Tile
     int pos = m - b * p.rows_per_batch;
     if (pos >= __ldg(p.row_lens + b)) return -1;
   }
+  if (p.grp != nullptr && __ldg(p.grp + m / p.rows_per_batch) != t.g) return -1;   // another group's N block
   return m;
 }
 
@@ -312,6 +343,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
   const int arow = q * 32 + lane;
   const long long orow = output_row(p, t, arow);
   const int n0_tile = t.n0;
+  const int oshift = t.g * p.group_n;   // grouped output: columns of group g start at output column 0
   if (p.debug_skip_epi == 1) return;  // main-loop-only timing: wrong results by construction (2: everything but the stores)
   if constexpr (EPI == EPI_LSE) {
     // log-sum-exp partial of x = acc + bias over this thread's columns [c0, c1) of the tile (one 128-column slab when
@@ -480,7 +512,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
       const long long o = __shfl_sync(0xffffffffu, orow, it * 4 + rsub);
-      ro[it] = (o >= 0) ? o * p.ldo + n0_tile + slot * 8 : -1;
+      ro[it] = (o >= 0) ? o * p.ldo + n0_tile - oshift + slot * 8 : -1;
     }
     bf16* out = reinterpret_cast<bf16*>(p.out);
     uint32_t* stage_u = reinterpret_cast<uint32_t*>(stage);
@@ -591,7 +623,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
           if (n0_tile + cc >= p.N) break;
           uint32_t acc[32];
           acc_ld32<BN>(accs, arow, cc, acc);
-          if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + cc, acc);
+          if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + cc, oshift, acc);
         }
       }
     }
@@ -601,7 +633,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
       const long long o = __shfl_sync(0xffffffffu, orow, it * 4 + rsub);
-      ro[it] = (o >= 0) ? o * p.ldo + n0_tile + slot * 4 : -1;
+      ro[it] = (o >= 0) ? o * p.ldo + n0_tile - oshift + slot * 4 : -1;
     }
     float* out = reinterpret_cast<float*>(p.out);
     float4 r[8];
@@ -672,7 +704,7 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       if (n0_tile + c >= p.N) break;
       uint32_t acc[32];
       acc_ld32<BN>(accs, arow, c, acc);
-      if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + c, acc);
+      if (orow >= 0) store_chunk<EPI>(p, orow, n0_tile + c, oshift, acc);
     }
   }
 }
@@ -754,6 +786,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == 0 && lane == 0) {
       uint32_t stage = 0, phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        if (!tile_active(p, tile, BN)) continue;
         TileCoord t = decode_tile(p, tile, BN);
         for (int kbx = 0; kbx < nkb; ++kbx) {
           // bf16x3: pass 0 = A_hi W_hi, pass 1 = A_lo W_hi, pass 2 = A_hi W_lo
@@ -786,8 +819,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // one warpgroup drains at a time: warp wl takes rows [32 wl, 32 wl + 32) and all columns
     float* stage_w = stage_epi + wl * 1024;
     float acc[BN];   // rows 0-63 in acc[0, BN/2), rows 64-127 in acc[BN/2, BN) (wgmma fragment layout, common.cuh)
-    for (int i = wg; blockIdx.x + i * gridDim.x < p.num_tiles; i += kConsumerWGs) {
-      const int tile = blockIdx.x + i * gridDim.x;
+    // i counts the CTA's active tiles (tile_active), the producer's ring order; tile i belongs to warpgroup i % 2
+    int active = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      if (!tile_active(p, tile, BN)) continue;
+      const int i = active++;
+      if (i % kConsumerWGs != wg) continue;
       TileCoord t = decode_tile(p, tile, BN);
       // the ring is consumed in the CTA's tile order: tile i's k-blocks are ring uses [i * nkb, (i + 1) * nkb)
       const uint32_t u0 = (uint32_t)i * (uint32_t)nkb;
@@ -1070,14 +1107,14 @@ static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
     default: kern = gemm_wg_kernel<BN, EPI_GENERIC, false>; break;
   }
   RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES));
-  p.tiles_n = (a.N + BN - 1) / BN;
+  p.tiles_n = a.grp ? p.grp_slots * (p.group_n / BN) : (a.N + BN - 1) / BN;
   int tiles_m = a.conv_mode ? a.conv_B * a.conv_F2 * p.conv_tt : (a.M + 127) / 128;
   p.num_tiles = tiles_m * p.tiles_n;
   int grid = p.num_tiles < g_num_sms ? p.num_tiles : g_num_sms;
   GemmProfRec rec;
   if (g_prof_on) {
     if (prof_event(&rec.a) || prof_event(&rec.b)) return -1;
-    rec.flops = 2.0 * (double)a.M * (double)a.N * (double)a.K * (a.x3 ? 3.0 : 1.0);
+    rec.flops = 2.0 * (double)a.M * (double)(a.grp ? a.group_n : a.N) * (double)a.K * (a.x3 ? 3.0 : 1.0);
     RVB_CHECK_CUDA(cudaEventRecord(rec.a, stream));
   }
   kern<<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
@@ -1123,7 +1160,20 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   p.act = a.act;
   p.out_mode = a.out_mode;
   p.out = a.out;
-  p.ldo = a.ldo ? a.ldo : (long long)(a.act == ACT_GLU ? a.N / 2 : a.N) * (a.out_split > 0 ? 2 : 1);
+  if (a.grp) {
+    RVB_REQUIRE(a.group_n > 0 && a.group_n % 64 == 0 && a.N % a.group_n == 0 && a.rows_per_batch > 0 &&
+                    a.act == ACT_NONE && (a.out_mode == OUT_BF16 || a.out_mode == OUT_F32) && !a.conv_mode && !a.rp_pos,
+                "gemm: a grouped output needs group_n %% 64 == 0 dividing N (N=%d group_n=%d), rows_per_batch, no "
+                "activation and a plain bf16 / fp32 output", a.N, a.group_n);
+    RVB_REQUIRE(get_gemm_impl() != 1, "gemm: grouped output is not built for the simt bring-up kernel");
+  }
+  p.grp = a.grp;
+  p.group_n = a.grp ? a.group_n : a.N;
+  if (a.grp) {   // rows [r0, r0 + 128) touch at most 127 / rpb + 2 utterances
+    const int rpb = a.rows_per_batch, n_utt = (a.M + rpb - 1) / rpb;
+    p.grp_slots = std::min(n_utt, 127 / rpb + 2);
+  }
+  p.ldo = a.ldo ? a.ldo : (long long)(a.act == ACT_GLU ? a.N / 2 : p.group_n) * (a.out_split > 0 ? 2 : 1);
   p.alpha = a.alpha;
   p.row_lens = a.row_lens;
   p.rows_per_batch = a.rows_per_batch > 0 ? a.rows_per_batch : a.M;
@@ -1208,7 +1258,10 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   if (get_encode_fn()) return -1;
   // 64-wide tiles for narrow outputs; RVB_GEMM=narrow (impl 2) takes them for every shape whose epilogue allows it:
   // all but the log-sum-exp partials (128-column slabs) and GLU hi/lo pairs (written 128 accumulator columns at a time)
-  const bool narrow = a.N <= 64 || (get_gemm_impl() == 2 && a.out_mode != OUT_LSE && !(a.act == ACT_GLU && a.out_split > 0));
+  // (a grouped output takes the tiles a plain launch of one group's N columns would take)
+  const bool narrow = p.group_n <= 64 || (get_gemm_impl() == 2 && a.out_mode != OUT_LSE && !(a.act == ACT_GLU && a.out_split > 0));
+  RVB_REQUIRE(!a.grp || p.group_n % (narrow ? 64 : 128) == 0, "gemm: grouped output needs group_n %% %d == 0 (group_n=%d)",
+              narrow ? 64 : 128, p.group_n);
   if (!narrow) return launch_wg<128>(a, p, stream);
   return launch_wg<64>(a, p, stream);
 }

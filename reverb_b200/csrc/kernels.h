@@ -77,6 +77,13 @@ struct GemmArgs {
   const int* lse_gather = nullptr;   // (M) column index per row, < 0 = none
   float2* lse_part = nullptr;        // (M, lse_slabs(N)) {max, sum exp(x - max)}; slabs without columns hold {-inf, 0}
   float* lse_tgt = nullptr;          // (M) the gathered x
+  // grouped output (language-specific linears with per-utterance mixing weights): W (N, K) and bias (N) stack N / group_n
+  // blocks of group_n rows, one per group.  Row m belongs to utterance m / rows_per_batch and takes only the block of its
+  // group g = grp[m / rows_per_batch] (int32, device), written at output column n - g * group_n (ldo 0 -> group_n).
+  // Every element equals a plain launch of that group's block: same tile width, k-block order and epilogue.  Tiles whose
+  // rows hold no utterance of their block's group are skipped.  act none, out_mode OUT_BF16 (or its pair) / OUT_F32.
+  const int* grp = nullptr;
+  int group_n = 0;
 };
 // out[m] = gather[m] >= 0 ? tgt[m] - logsumexp(partials of row m) : 0
 int launch_lse_merge(const float2* part, int slabs, const float* tgt, const int* gather, int M, float* out,

@@ -195,6 +195,8 @@ class Engine:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def _cat(self, cat_embs) -> Tuple[Optional[np.ndarray], int]:
+        """cat_embs (num_langs,) or (B, num_langs), one row per utterance -> (flat float32 array, n_cat); the native
+        call checks n_cat against both lengths."""
         if self.num_langs == 0:
             return None, 0
         if cat_embs is None:

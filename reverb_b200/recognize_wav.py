@@ -48,8 +48,9 @@ def get_args(argv=None):
                    help="right to left weight for attention rescoring decode mode")
     p.add_argument("--overwrite_cmvn", action="store_true",
                    help="overwrite CMVN params in model with those in config file")
-    p.add_argument("--verbatimicity", type=float, default=1.0,
-                   help="0.0 = nonverbatim ... 1.0 = verbatim; passed to the language-specific layers")
+    p.add_argument("--verbatimicity", type=float, nargs="+", default=1.0,
+                   help="0.0 = nonverbatim ... 1.0 = verbatim; passed to the language-specific layers.  One value, or "
+                        "one per --audio_file")
     p.add_argument("--timings_adjustment", type=float, default=230,
                    help="Subtract timings_adjustment milliseconds from each timestamp")
     p.add_argument("--context_list_path", default=None,
@@ -63,7 +64,14 @@ def get_args(argv=None):
     p.add_argument("--diarization_synthetic", action="store_true",
                    help="Like --diarization_model, with the seeded synthetic diarization weights")
     p.add_argument("--log_level", choices=["DEBUG", "INFO", "WARNING", "ERROR", "CRITICAL"], default="INFO")
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    if isinstance(args.verbatimicity, list):           # one value stays a float; else one per --audio_file
+        if len(args.verbatimicity) not in (1, len(args.audio_file)):
+            p.error(f"--verbatimicity takes one value or one per --audio_file ({len(args.audio_file)}), "
+                    f"got {len(args.verbatimicity)}")
+        if len(args.verbatimicity) == 1:
+            args.verbatimicity = args.verbatimicity[0]
+    return args
 
 
 def output_names(audio_files) -> list:

@@ -200,7 +200,7 @@ class ReverbASR:
             pass
         return outputs
 
-    def transcribe_files(self, audio_files, modes: List[str], format: str = "txt", verbatimicity: float = 1.0,
+    def transcribe_files(self, audio_files, modes: List[str], format: str = "txt", verbatimicity=1.0,
                          chunk_size: int = 2051, batch_size: int = 1, beam_size: int = 10,
                          decoding_chunk_size: int = -1, num_decoding_left_chunks: int = -1, ctc_weight: float = 0.1,
                          simulate_streaming: bool = False, reverse_weight: float = 0.0, blank_penalty: float = 0.0,
@@ -209,6 +209,9 @@ class ReverbASR:
         """Transcribes many recordings with one set of decode settings -> (audio_file, [output per mode]) in input
         order, each as soon as it and every earlier recording are decoded.  Every output is the one
         `transcribe_modes(audio_file, ...)` gives on its own.
+
+        verbatimicity: one value for every file, or a sequence with one value per file (0.0 = nonverbatim ... 1.0 =
+        verbatim).  Files with different values still share batches: each chunk's row carries its file's value.
 
         Batches hold chunks of several recordings, and tail chunks run at a trimmed length (reverb_b200/corpus.py,
         DESIGN.md §4f).  Files are read and parsed on a background thread, one window of recordings ahead; upload,
@@ -221,6 +224,13 @@ class ReverbASR:
         recognize_wav (CTM) -> words2speakers writes, byte for byte.  Diarization runs once per recording, on all of its
         channels downmixed (infer.read_audio; the ASR reads channel 0), on the caller's thread and current stream as
         the recording is yielded."""
+        audio_files = list(audio_files)
+        per_file = isinstance(verbatimicity, (list, tuple, np.ndarray, torch.Tensor))
+        if per_file:                      # fail before any audio is read
+            verbatimicity = [float(v) for v in verbatimicity]
+            if len(verbatimicity) != len(audio_files):
+                raise ValueError(f"verbatimicity has {len(verbatimicity)} values for {len(audio_files)} audio files; "
+                                 "give one value, or one per file")
         if (format == "stm") != (diarization is not None):   # fail before any audio is read
             raise ValueError('format="stm" and diarization= go together: a speaker-attributed transcript needs a '
                              'SpeakerDiarization, and only format="stm" uses one')
@@ -233,19 +243,29 @@ class ReverbASR:
         # mask, and the attention mode's beam search runs up to T' steps
         trim = not simulate_streaming and "attention" not in modes
         right = corpus.right_context(self.configs["encoder_conf"])
-        cat_embs = torch.tensor([verbatimicity, 1.0 - verbatimicity])
+        cat_embs = None if per_file else torch.tensor([verbatimicity, 1.0 - verbatimicity])
         kw = dict(decoding_chunk_size=decoding_chunk_size, num_decoding_left_chunks=num_decoding_left_chunks,
                   ctc_weight=ctc_weight, simulate_streaming=simulate_streaming, reverse_weight=reverse_weight,
                   context_graph=context_graph, blank_id=self.blank_id, blank_penalty=blank_penalty,
                   length_penalty=length_penalty, infos={"tasks": ["transcribe"], "langs": ["en"]}, cat_embs=cat_embs)
 
         def decode_batch(model, batch):
-            return model.decode(modes, batch[0], batch[1], beam_size, **kw)
+            return model.decode(modes, batch[0], batch[1], beam_size, **(kw if len(batch) == 2 else
+                                                                        dict(kw, cat_embs=batch[2])))
+
+        first = [0]                          # input index of the next recording the reader hands over
 
         def window_batches(window):
-            return self._window_batches(window, chunk_size, batch_size, right, trim)
+            jobs = self._window_batches(window, chunk_size, batch_size, right, trim)
+            if not per_file:
+                return jobs
+            v = verbatimicity[first[0]:first[0] + len(window)]
+            first[0] += len(window)
+            # one [v, 1 - v] row per chunk, built as the single-file call builds its vector
+            return [(plan, fb, fl, torch.tensor([[v[r], 1.0 - v[r]] for r, _ in plan.slots]))
+                    for plan, fb, fl in jobs]
 
-        reader = _Reader(self, list(audio_files), corpus.window_frames(batch_size, chunk_size))
+        reader = _Reader(self, audio_files, corpus.window_frames(batch_size, chunk_size))
         waiting: deque = deque()             # recordings not yet yielded, in input order
         stream = None
         try:
@@ -255,17 +275,17 @@ class ReverbASR:
                     for window in reader:
                         waiting.extend(window)
                         jobs = window_batches(window)
-                        for (plan, _, _), res in zip(jobs, self._lanes.run([job[1:] for job in jobs], decode_batch)):
-                            yield (plan, window), res
+                        for job, res in zip(jobs, self._lanes.run([job[1:] for job in jobs], decode_batch)):
+                            yield (job[0], window), res
             else:
                 plans: deque = deque()
 
                 def batches():
                     for window in reader:
                         waiting.extend(window)
-                        for plan, fb, fl in window_batches(window):
+                        for plan, *batch in window_batches(window):
                             plans.append((plan, window))
-                            yield fb, fl
+                            yield tuple(batch)
 
                 # one software-pipelined decode_stream across window boundaries
                 stream = self.model.decode_stream(batches(), modes, beam_size, **kw)
