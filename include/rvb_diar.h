@@ -5,7 +5,8 @@
  * requirements.txt:1).  There is no FFI in the reference for this path; these are the entry points a binding of
  * `pyannote.audio.Model.__call__` for the segmentation / embedding models would replace:
  *
- *   rvb_seg_*  PyanNet segmentation: waveform windows -> per-frame log-probabilities over the powerset classes
+ *   rvb_seg_*        PyanNet segmentation (v1): waveform windows -> per-frame log-probabilities over the powerset classes
+ *   rvb_wavlm_seg_*  WavLM segmentation (v2), same outputs
  *   rvb_emb_*  WeSpeaker ResNet34 speaker embedding: waveform windows (+ per-frame weights) -> 256-d vectors
  *
  * ** parity unpinned **: pyannote's source and the model weights are not available offline (SURVEY.md §8c-iii); the
@@ -52,6 +53,55 @@ RVB_API int rvb_seg_num_frames(const rvb_seg_model* m, int num_samples);
  * d_sincnet (optional, B x frames x conv_channels): the SincNet output, for staged parity tests. */
 RVB_API int rvb_seg_forward(rvb_seg_model* m, const float* d_wave, int B, int num_samples, float* d_logp,
                             float* d_sincnet, void* stream);
+
+/* ---- WavLM segmentation (reverb-diarization-v2: pyannote SSeRiouSS on WavLM Base) --------------------------------
+ * waveform window -> torchaudio wavlm_base() conv feature extractor (GroupNorm on layer 0), feature projection,
+ * positional conv, the transformer's LayerNorm, 12 post-LN transformer layers with gated relative-position bias -> softmax(wav2vec_weights)-weighted
+ * sum of the 12 layer outputs -> PyanNet's head (bidirectional LSTM, linears, classifier, log_softmax).
+ * Receptive field 400 samples, step 320.  bf16 tensor-core GEMMs and attention, fp32 residual stream, norms and head.
+ * Workspace: about 100 MB per 10 s window (the layer-0 output alone is 32.8 MB in bf16), grow-only; a call runs its
+ * windows 32 at a time, which bounds it at about 3.2 GB. */
+typedef struct rvb_wavlm_seg_model rvb_wavlm_seg_model;
+
+typedef struct rvb_wavlm_seg_config {
+  int sample_rate;      /* 16000 */
+  int conv_channels;    /* 512 (the only width built) */
+  int embed_dim;        /* 768 */
+  int num_layers;       /* 12 */
+  int num_heads;        /* 12, 64 wide */
+  int ffn_dim;          /* 3072 */
+  int pos_conv_kernel;  /* 128 (even: the last output frame is dropped) */
+  int pos_conv_groups;  /* 16 */
+  int num_buckets;      /* 320 relative-position buckets (bidirectional) */
+  int max_distance;     /* 800 */
+  int lstm_hidden;      /* 128, bidirectional */
+  int lstm_layers;      /* 4 */
+  int linear_dim;       /* 128 */
+  int linear_layers;    /* 2 */
+  int num_classes;      /* 7 powerset classes */
+} rvb_wavlm_seg_config;
+
+RVB_API rvb_wavlm_seg_model* rvb_wavlm_seg_create(const rvb_wavlm_seg_config* cfg);
+/* fp32 host tensors under pyannote's state_dict names: wav2vec.<torchaudio wavlm_base names> (the positional conv's
+ * weight norm as parametrizations.weight.original0 / original1 or weight_g / weight_v), wav2vec_weights,
+ * lstm.*_l{k}[_reverse], linear.{i}.*, classifier.*.  Unknown names are rejected here; missing or mis-sized tensors at
+ * finalize. */
+RVB_API int rvb_wavlm_seg_set_tensor(rvb_wavlm_seg_model* m, const char* name, const float* host, long long count);
+RVB_API int rvb_wavlm_seg_finalize(rvb_wavlm_seg_model* m);
+RVB_API void rvb_wavlm_seg_destroy(rvb_wavlm_seg_model* m);
+/* output frames for a window of num_samples (160000 -> 499; 0 below 400) */
+RVB_API int rvb_wavlm_seg_num_frames(const rvb_wavlm_seg_model* m, int num_samples);
+/* d_wave (B, num_samples) fp32 -> d_logp (B, frames, num_classes) fp32 log-probabilities.  Optional, for staged tests:
+ * d_conv (B, frames, conv_channels) the conv extractor output, d_layers (num_layers, B, frames, embed_dim) every
+ * transformer layer's output. */
+RVB_API int rvb_wavlm_seg_forward(rvb_wavlm_seg_model* m, const float* d_wave, int B, int num_samples, float* d_logp,
+                                  float* d_conv, float* d_layers, void* stream);
+/* For tests and tools: the wgmma attention with WavLM's gated relative-position bias, as the forward runs it (d_k = 64,
+ * self-attention, Tq = Tk = T).  Group g owns rows [g*T, (g+1)*T) of q / k / v / out (bf16, pointers at head 0);
+ * score(i, j) = q_i . k_j * scale + d_gate[(g*H + h)*T + i] * d_rel_bias[h*(2T - 1) + j - i + T - 1] (fp32). */
+RVB_API int rvb_attention_tc_relbias(const void* d_q, const void* d_k, const void* d_v, void* d_out, int ldq, int ldk,
+                                     int ldv, int ldo, int groups, int T, int H, const float* d_gate,
+                                     const float* d_rel_bias, float scale, void* stream);
 
 /* ---- WeSpeaker ResNet34 speaker embedding ------------------------------------------------------------------------
  * waveform window in [-1, 1] -> x 2^15 -> Kaldi fbank (80 mel, hamming window, 25 / 10 ms, no dither) -> minus the mean

@@ -29,6 +29,14 @@ class SegConfig(C.Structure):
         "lstm_layers", "linear_dim", "linear_layers", "num_classes")]
 
 
+class WavlmSegConfig(C.Structure):
+    """Mirror of `rvb_wavlm_seg_config` (include/rvb_diar.h)."""
+    _fields_ = [(n, C.c_int) for n in (
+        "sample_rate", "conv_channels", "embed_dim", "num_layers", "num_heads", "ffn_dim", "pos_conv_kernel",
+        "pos_conv_groups", "num_buckets", "max_distance", "lstm_hidden", "lstm_layers", "linear_dim", "linear_layers",
+        "num_classes")]
+
+
 class EmbConfig(C.Structure):
     """Mirror of `rvb_emb_config` (include/rvb_diar.h)."""
     _fields_ = [("sample_rate", C.c_int), ("num_mel_bins", C.c_int), ("m_channels", C.c_int), ("embed_dim", C.c_int),
@@ -112,6 +120,13 @@ SIGNATURES = {
     "rvb_seg_destroy": (None, [_vp]),
     "rvb_seg_num_frames": (_i, [_vp, _i]),
     "rvb_seg_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "rvb_wavlm_seg_create": (_vp, [C.POINTER(WavlmSegConfig)]),
+    "rvb_wavlm_seg_set_tensor": (_i, [_vp, C.c_char_p, _vp, _ll]),
+    "rvb_wavlm_seg_finalize": (_i, [_vp]),
+    "rvb_wavlm_seg_destroy": (None, [_vp]),
+    "rvb_wavlm_seg_num_frames": (_i, [_vp, _i]),
+    "rvb_wavlm_seg_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "rvb_attention_tc_relbias": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _f, _vp]),
     "rvb_emb_create": (_vp, [C.POINTER(EmbConfig)]),
     "rvb_emb_set_tensor": (_i, [_vp, C.c_char_p, _vp, _ll]),
     "rvb_emb_finalize": (_i, [_vp]),

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librvb_b200.so")
 SOURCES = ["gemm.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "attention_f32.cu", "fbank.cu", "resample.cu", "ctc.cu",
-           "context.cu", "align.cu", "engine.cu", "diar_seg.cu", "diar_emb.cu",
+           "context.cu", "align.cu", "engine.cu", "diar_seg.cu", "diar_wavlm.cu", "diar_emb.cu",
            "diar_cluster.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]

@@ -56,6 +56,9 @@ struct AttnTcParams {
   const uint32_t* key_bits;  // optional per-(query row, key) visibility bits (AttnTcArgs::key_bits)
   int bits_ld;
   float scale_log2;
+  // MASK_RELB: gated relative-position bias gate[(g*H + h)*Tq + i] * rel_bias[h*(2Tk-1) + j - i + Tk - 1], Tq == Tk
+  const float* gate;
+  const float* rel_bias;
 };
 
 // Which masks a launch applies on top of the key lengths.  Each kind is its own instantiation, so the encoder's
@@ -64,6 +67,7 @@ enum AttnMask : int {
   MASK_LENS = 0,   // key lengths only (encoder self-attention, cross-attention)
   MASK_CHUNK = 1,  // chunk / causal mask, p.chunk > 0
   MASK_BITS = 2,   // key_bits, and the chunk / causal mask when p.chunk > 0 (prefix-tree self-attention)
+  MASK_RELB = 3,   // key lengths + WavLM's gated relative-position bias (the head's table staged in shared memory)
 };
 
 // one S = Q . K''^T tile product into s (not committed)
@@ -90,6 +94,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   uint64_t* v_empty = v_full + AT_ST;      // [AT_ST]
   static_assert(1 + 4 * AT_ST <= 32, "barrier block is 256 bytes");
   float* s_bias = reinterpret_cast<float*>(bars + 32);   // [ntiles * AT_BN]: key bias * scale*log2e, -inf when masked
+  float* s_rb = s_bias + (p.Tk + AT_BN - 1) / AT_BN * AT_BN;             // MASK_RELB: [2Tk - 1] rel_bias row of the head * log2e
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qtile = blockIdx.x, h = blockIdx.y, g = blockIdx.z;
@@ -137,6 +142,10 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       const int key = jt0 * AT_BN + kk;
       s_bias[kk] = (key < klen) ? (kb ? __ldg(kb + key) * p.scale_log2 : 0.f) : -INFINITY;
     }
+    if (MASK == MASK_RELB) {
+      const float* rb = p.rel_bias + (long long)h * (2 * p.Tk - 1);
+      for (int d = threadIdx.x; d < 2 * p.Tk - 1; d += AT_THREADS) s_rb[d] = __ldg(rb + d) * 1.4426950408889634f;
+    }
   }
   __syncthreads();
 
@@ -146,6 +155,11 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int rloc = wg * 64 + wl * 16 + (lane >> 2);
   const int row[2] = {q0 + rloc, q0 + rloc + 8};
   const int cq = 2 * (lane & 3);
+  float gate[2] = {0.f, 0.f};
+  if (MASK == MASK_RELB) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) gate[i] = __ldg(p.gate + ((long long)g * p.H + h) * p.Tq + min(row[i], p.Tq - 1));
+  }
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -188,6 +202,20 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       for (int i = 0; i < 2; ++i) {
         s[4 * jj + 2 * i] = fmaf(s[4 * jj + 2 * i], p.scale_log2, b2.x);
         s[4 * jj + 2 * i + 1] = fmaf(s[4 * jj + 2 * i + 1], p.scale_log2, b2.y);
+      }
+    }
+    if (MASK == MASK_RELB) {
+      // masked keys are -inf already; the table index is clamped for them and for rows past Tq
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int d0 = kbase - row[i] + p.Tk - 1;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int d = min(max(d0 + 8 * jj + cq + c, 0), 2 * p.Tk - 2);
+            s[4 * jj + 2 * i + c] = fmaf(gate[i], s_rb[d], s[4 * jj + 2 * i + c]);
+          }
       }
     }
     if (chunked) {
@@ -417,6 +445,8 @@ static int attn_mask_kind(bool chunk_or_causal, bool key_bits) {
 // Q, both rings, barriers and the key-bias row: 86 272 B at Tk = 748.  Two CTAs fit the 228 KB of an SM (1 KB of it
 // reserved per CTA) up to Tk = 8 128; longer key rows run one CTA per SM.
 static size_t attn_smem_bytes(int Tk) { return AT_SMEM_FIXED + (size_t)((Tk + AT_BN - 1) / AT_BN) * AT_BN * sizeof(float); }
+// MASK_RELB also stages the head's (2 Tk - 1)-entry bias table
+static size_t attn_relb_smem_bytes(int Tk) { return attn_smem_bytes(Tk) + (size_t)(2 * Tk) * sizeof(float); }
 
 template <int MASK>
 static int attn_opt_in(size_t smem) {
@@ -457,6 +487,9 @@ int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
               "attention_tc: operands must be 16-byte aligned");
   RVB_REQUIRE((!a.causal && a.chunk <= 0) || a.Tq == a.Tk, "attention_tc: causal / chunk masks need Tq == Tk");
   RVB_REQUIRE(!(a.causal && a.chunk > 0), "attention_tc: causal and chunk mask are exclusive");
+  const bool relb = a.rel_bias != nullptr;
+  RVB_REQUIRE(!relb || (a.gate && a.Tq == a.Tk && !a.causal && a.chunk <= 0 && !a.key_bits && !a.key_bias),
+              "attention_tc: the gated relative-position bias needs a gate, Tq == Tk and no other mask or key bias");
   if (a.groups <= 0 || a.Tq <= 0) return 0;
   if (g_encode_att == nullptr) {
     void* fn = nullptr;
@@ -479,15 +512,18 @@ int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream) {
   p.bits_ld = a.bits_ld;
   RVB_REQUIRE(a.key_bits == nullptr || a.bits_ld >= 2 * ((a.Tk + 63) / 64), "attention_tc: key_bits rows are too short");
   p.scale_log2 = a.scale * 1.4426950408889634f;
+  p.gate = a.gate;
+  p.rel_bias = a.rel_bias;
   CUtensorMap tmQ, tmK, tmV;
   if (tmap_2d(&tmQ, a.q, (long long)a.H * AT_DK, (long long)a.groups * a.Tq, a.ldq, AT_BM)) return -1;
   if (tmap_2d(&tmK, a.k, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldk, AT_BN)) return -1;
   if (tmap_2d(&tmV, a.v, (long long)a.H * AT_DK, (long long)a.groups * a.Tk, a.ldv, AT_BN)) return -1;
   dim3 grid((a.Tq + AT_BM - 1) / AT_BM, a.H, a.groups);
-  const size_t smem = attn_smem_bytes(a.Tk);
+  const size_t smem = relb ? attn_relb_smem_bytes(a.Tk) : attn_smem_bytes(a.Tk);
   RVB_REQUIRE(smem <= 227 * 1024, "attention_tc: Tk=%d needs %zu B of shared memory", a.Tk, smem);
   int rc;
-  switch (attn_mask_kind(a.causal || a.chunk > 0, a.key_bits != nullptr)) {
+  switch (relb ? (int)MASK_RELB : attn_mask_kind(a.causal || a.chunk > 0, a.key_bits != nullptr)) {
+    case MASK_RELB: rc = attn_launch<MASK_RELB>(grid, smem, stream, tmQ, tmK, tmV, p); break;
     case MASK_LENS: rc = attn_launch<MASK_LENS>(grid, smem, stream, tmQ, tmK, tmV, p); break;
     case MASK_CHUNK: rc = attn_launch<MASK_CHUNK>(grid, smem, stream, tmQ, tmK, tmV, p); break;
     default: rc = attn_launch<MASK_BITS>(grid, smem, stream, tmQ, tmK, tmV, p); break;

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 #include <atomic>
 
@@ -80,6 +81,24 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + __expf(-x)); }
+// torch's default (erf) GELU
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+
+// host fp32 <-> bf16 bits (round to nearest even, NaN kept)
+static inline uint16_t f2bf(float f) {
+  uint32_t u;
+  memcpy(&u, &f, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);  // NaN
+  u += 0x7fffu + ((u >> 16) & 1u);                                            // round to nearest even
+  return (uint16_t)(u >> 16);
+}
+
+static inline float bf2f(uint16_t h) {
+  uint32_t u = (uint32_t)h << 16;
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+}
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);

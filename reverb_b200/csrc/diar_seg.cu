@@ -339,10 +339,7 @@ struct rvb_seg_model {
   float* norm_b[3] = {nullptr, nullptr, nullptr};
   float* conv_w[2] = {nullptr, nullptr};
   float* conv_b[2] = {nullptr, nullptr};
-  std::vector<float*> wih, whh, lbias;   // per layer: (2*4H, in), (2, 4H, H), (2*4H)
-  std::vector<float*> lin_w, lin_b;
-  float* cls_w = nullptr;
-  float* cls_b = nullptr;
+  rvb::SegHead head;
   rvb::DevBuf ws_a, ws_b, ws_g, ws_h0, ws_h1;
 };
 
@@ -391,6 +388,85 @@ static int seg_frames(const rvb_seg_config& c, int num_samples, int* l1, int* l2
   if (l2) *l2 = b;
   if (l3) *l3 = d;
   return d;
+}
+
+int seg_head_load(WeightStore& store, int in_dim, SegHead* h) {
+  const std::vector<float>* t = nullptr;
+  const std::vector<float>* t2 = nullptr;
+  const int H = h->hidden;
+  for (int l = 0; l < h->lstm_layers; ++l) {
+    const int in = l == 0 ? in_dim : 2 * H;
+    std::vector<float> wih((size_t)2 * 4 * H * in), whh((size_t)2 * 4 * H * H), bias((size_t)2 * 4 * H);
+    for (int d = 0; d < 2; ++d) {
+      const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
+      if (store.need("lstm.weight_ih" + sfx, (size_t)4 * H * in, &t)) return -1;
+      memcpy(wih.data() + (size_t)d * 4 * H * in, t->data(), t->size() * sizeof(float));
+      if (store.need("lstm.weight_hh" + sfx, (size_t)4 * H * H, &t)) return -1;
+      memcpy(whh.data() + (size_t)d * 4 * H * H, t->data(), t->size() * sizeof(float));
+      if (store.need("lstm.bias_ih" + sfx, (size_t)4 * H, &t) ||
+          store.need("lstm.bias_hh" + sfx, (size_t)4 * H, &t2))
+        return -1;
+      for (int i = 0; i < 4 * H; ++i) bias[(size_t)d * 4 * H + i] = (*t)[i] + (*t2)[i];
+    }
+    float *a = nullptr, *b = nullptr, *cc = nullptr;
+    if (store.upload(wih.data(), wih.size(), &a) || store.upload(whh.data(), whh.size(), &b) ||
+        store.upload(bias.data(), bias.size(), &cc))
+      return -1;
+    h->wih.push_back(a);
+    h->whh.push_back(b);
+    h->lbias.push_back(cc);
+  }
+  int in = 2 * H;
+  for (int i = 0; i < h->linear_layers; ++i) {
+    const std::string p = "linear." + std::to_string(i);
+    float *a = nullptr, *b = nullptr;
+    if (store.need(p + ".weight", (size_t)h->linear_dim * in, &t) || store.upload(t->data(), t->size(), &a))
+      return -1;
+    if (store.need(p + ".bias", h->linear_dim, &t) || store.upload(t->data(), t->size(), &b)) return -1;
+    h->lin_w.push_back(a);
+    h->lin_b.push_back(b);
+    in = h->linear_dim;
+  }
+  if (store.need("classifier.weight", (size_t)h->num_classes * in, &t) ||
+      store.upload(t->data(), t->size(), &h->cls_w))
+    return -1;
+  if (store.need("classifier.bias", h->num_classes, &t) || store.upload(t->data(), t->size(), &h->cls_b))
+    return -1;
+  return 0;
+}
+
+int seg_head_forward(const SegHead& h, const float* x, int in_dim, int B, int T, float* g, float* h0, float* h1,
+                     float* y0, float* y1, float* logp, cudaStream_t stream) {
+  const int H = h.hidden;
+  // LSTM stack
+  const long long M = (long long)B * T;
+  const float* xin = x;
+  int in = in_dim;
+  float* hbuf[2] = {h0, h1};
+  for (int l = 0; l < h.lstm_layers; ++l) {
+    float* hout = hbuf[l & 1];   // layer 0 reads x (may be h1) and writes h0, layer 1 reads h0 and writes h1, ...
+    if (launch_sgemm(xin, in, h.wih[l], in, h.lbias[l], g, 8 * H, (int)M, 8 * H, in, 0, stream)) return -1;
+    dim3 grid(2 * ((B + LS_BT - 1) / LS_BT), 2);
+    lstm_rec_kernel<<<grid, LS_THREADS, 0, stream>>>(g, h.whh[l], hout, B, T);
+    RVB_COUNT_LAUNCH();
+    RVB_CHECK_LAUNCH();
+    xin = hout;
+    in = 2 * H;
+  }
+  // linear stack + classifier + log_softmax
+  const float* cur = xin;
+  for (int i = 0; i < h.linear_layers; ++i) {
+    float* dst = (i & 1) ? y1 : y0;
+    if (launch_sgemm(cur, in, h.lin_w[i], in, h.lin_b[i], dst, h.linear_dim, (int)M, h.linear_dim, in, 1, stream)) return -1;
+    cur = dst;
+    in = h.linear_dim;
+  }
+  float* logits = (cur == y0) ? y1 : y0;
+  if (launch_sgemm(cur, in, h.cls_w, in, h.cls_b, logits, h.num_classes, (int)M, h.num_classes, in, 0, stream)) return -1;
+  logsoftmax_rows_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(logits, logp, M, h.num_classes);
+  RVB_COUNT_LAUNCH();
+  RVB_CHECK_LAUNCH();
+  return 0;
 }
 
 }  // namespace rvb
@@ -451,45 +527,12 @@ RVB_API int rvb_seg_finalize(rvb_seg_model* m) {
     if (m->store.need(p + ".bias", c.conv_channels, &t) || m->store.upload(t->data(), t->size(), &m->conv_b[i]))
       return -1;
   }
-  const int H = c.lstm_hidden;
-  for (int l = 0; l < c.lstm_layers; ++l) {
-    const int in = l == 0 ? c.conv_channels : 2 * H;
-    std::vector<float> wih((size_t)2 * 4 * H * in), whh((size_t)2 * 4 * H * H), bias((size_t)2 * 4 * H);
-    for (int d = 0; d < 2; ++d) {
-      const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
-      if (m->store.need("lstm.weight_ih" + sfx, (size_t)4 * H * in, &t)) return -1;
-      memcpy(wih.data() + (size_t)d * 4 * H * in, t->data(), t->size() * sizeof(float));
-      if (m->store.need("lstm.weight_hh" + sfx, (size_t)4 * H * H, &t)) return -1;
-      memcpy(whh.data() + (size_t)d * 4 * H * H, t->data(), t->size() * sizeof(float));
-      if (m->store.need("lstm.bias_ih" + sfx, (size_t)4 * H, &t) ||
-          m->store.need("lstm.bias_hh" + sfx, (size_t)4 * H, &t2))
-        return -1;
-      for (int i = 0; i < 4 * H; ++i) bias[(size_t)d * 4 * H + i] = (*t)[i] + (*t2)[i];
-    }
-    float *a = nullptr, *b = nullptr, *cc = nullptr;
-    if (m->store.upload(wih.data(), wih.size(), &a) || m->store.upload(whh.data(), whh.size(), &b) ||
-        m->store.upload(bias.data(), bias.size(), &cc))
-      return -1;
-    m->wih.push_back(a);
-    m->whh.push_back(b);
-    m->lbias.push_back(cc);
-  }
-  int in = 2 * H;
-  for (int i = 0; i < c.linear_layers; ++i) {
-    const std::string p = "linear." + std::to_string(i);
-    float *a = nullptr, *b = nullptr;
-    if (m->store.need(p + ".weight", (size_t)c.linear_dim * in, &t) || m->store.upload(t->data(), t->size(), &a))
-      return -1;
-    if (m->store.need(p + ".bias", c.linear_dim, &t) || m->store.upload(t->data(), t->size(), &b)) return -1;
-    m->lin_w.push_back(a);
-    m->lin_b.push_back(b);
-    in = c.linear_dim;
-  }
-  if (m->store.need("classifier.weight", (size_t)c.num_classes * in, &t) ||
-      m->store.upload(t->data(), t->size(), &m->cls_w))
-    return -1;
-  if (m->store.need("classifier.bias", c.num_classes, &t) || m->store.upload(t->data(), t->size(), &m->cls_b))
-    return -1;
+  m->head.hidden = c.lstm_hidden;
+  m->head.lstm_layers = c.lstm_layers;
+  m->head.linear_layers = c.linear_layers;
+  m->head.linear_dim = c.linear_dim;
+  m->head.num_classes = c.num_classes;
+  if (seg_head_load(m->store, c.conv_channels, &m->head)) return -1;
   m->store.drop_host();
   m->finalized = true;
   return 0;
@@ -560,36 +603,6 @@ RVB_API int rvb_seg_forward(rvb_seg_model* m, const float* d_wave, int B, int nu
   }
   if (d_sincnet)
     RVB_CHECK_CUDA(cudaMemcpyAsync(d_sincnet, x_lstm, (size_t)B * T * Cc * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  // LSTM stack
-  const long long M = (long long)B * T;
-  float* g = m->ws_g.as<float>();
-  const float* xin = x_lstm;
-  int in = Cc;
-  float* hbuf[2] = {m->ws_h0.as<float>(), m->ws_h1.as<float>()};
-  for (int l = 0; l < c.lstm_layers; ++l) {
-    float* hout = hbuf[l & 1];   // layer 0 reads h1 (x_lstm) and writes h0, layer 1 reads h0 and writes h1, ...
-    if (launch_sgemm(xin, in, m->wih[l], in, m->lbias[l], g, 8 * H, (int)M, 8 * H, in, 0, stream)) return -1;
-    dim3 grid(2 * ((B + LS_BT - 1) / LS_BT), 2);
-    lstm_rec_kernel<<<grid, LS_THREADS, 0, stream>>>(g, m->whh[l], hout, B, T);
-    RVB_COUNT_LAUNCH();
-    RVB_CHECK_LAUNCH();
-    xin = hout;
-    in = 2 * H;
-  }
-  // linear stack + classifier + log_softmax
-  float* y0 = m->ws_a.as<float>();
-  float* y1 = m->ws_b.as<float>();
-  const float* cur = xin;
-  for (int i = 0; i < c.linear_layers; ++i) {
-    float* dst = (i & 1) ? y1 : y0;
-    if (launch_sgemm(cur, in, m->lin_w[i], in, m->lin_b[i], dst, c.linear_dim, (int)M, c.linear_dim, in, 1, stream)) return -1;
-    cur = dst;
-    in = c.linear_dim;
-  }
-  float* logits = (cur == y0) ? y1 : y0;
-  if (launch_sgemm(cur, in, m->cls_w, in, m->cls_b, logits, c.num_classes, (int)M, c.num_classes, in, 0, stream)) return -1;
-  logsoftmax_rows_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(logits, d_logp, M, c.num_classes);
-  RVB_COUNT_LAUNCH();
-  RVB_CHECK_LAUNCH();
-  return 0;
+  return seg_head_forward(m->head, x_lstm, Cc, B, T, m->ws_g.as<float>(), m->ws_h0.as<float>(), x_lstm, m->ws_a.as<float>(),
+                          m->ws_b.as<float>(), d_logp, stream);
 }

@@ -37,21 +37,6 @@ void set_error(const char* fmt, ...) {
 }
 const char* last_error() { return g_err; }
 
-static inline uint16_t f2bf(float f) {
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);  // NaN
-  u += 0x7fffu + ((u >> 16) & 1u);                                            // round to nearest even
-  return (uint16_t)(u >> 16);
-}
-
-static inline float bf2f(uint16_t h) {
-  uint32_t u = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
-}
-
 struct Linear {  // bf16 weight (N, K) + fp32 bias (N) on device
   bf16* w = nullptr;
   float* b = nullptr;

@@ -141,11 +141,12 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 // Epilogue variants (compile-time): the hot combinations get straight-line code, everything else goes through the
 // generic runtime path.  EPI_GENERIC reads act / out_mode from the kernel parameters.
 enum Epi { EPI_BF16 = 0, EPI_BF16_RELU = 1, EPI_BF16_SILU = 2, EPI_F32 = 3, EPI_RESID = 4, EPI_GENERIC = 5, EPI_GLU = 6,
-           EPI_LSE = 7, EPI_BF16_RELPOS = 8 };
+           EPI_LSE = 7, EPI_BF16_RELPOS = 8, EPI_BF16_GELU = 9 };
 
 __host__ __device__ inline int select_epi(int act, int out_mode) {
   if (act == ACT_GLU) return EPI_GLU;
   if (out_mode == OUT_LSE) return EPI_LSE;
+  if (act == ACT_GELU) return EPI_BF16_GELU;   // bf16 output only (checked at launch)
   if (out_mode == OUT_BF16) return act == ACT_NONE ? EPI_BF16 : act == ACT_RELU ? EPI_BF16_RELU : EPI_BF16_SILU;
   if (act == ACT_NONE) return out_mode == OUT_F32 ? EPI_F32 : EPI_RESID;
   return EPI_GENERIC;
@@ -178,7 +179,7 @@ template <int EPI>
 __device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_row, int n0, int oshift, const uint32_t* acc) {
   float v[32];
   const bool full = (n0 + 32 <= p.N);
-  constexpr int OUT = (EPI <= EPI_BF16_SILU) ? OUT_BF16 : (EPI == EPI_F32) ? OUT_F32 : OUT_RESID_F32;
+  constexpr int OUT = (EPI <= EPI_BF16_SILU || EPI == EPI_BF16_GELU) ? OUT_BF16 : (EPI == EPI_F32) ? OUT_F32 : OUT_RESID_F32;
   const int out_mode = (EPI == EPI_GENERIC) ? p.out_mode : OUT;
   // bias (vectorised when the whole chunk is in range; bias + n0 is 16-byte aligned because n0 % 32 == 0)
   if (p.bias != nullptr) {
@@ -205,6 +206,9 @@ __device__ __forceinline__ void store_chunk(const GemmKParams& p, long long out_
   } else if (EPI == EPI_BF16_SILU) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = fast_silu(v[j]);
+  } else if (EPI == EPI_BF16_GELU) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
   } else if (EPI == EPI_GENERIC) {
     if (p.act == ACT_RELU) {
 #pragma unroll
@@ -503,7 +507,8 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
       acc_ld32<BN>(accs, arow, c + 32, gv);
       if (orow >= 0) store_glu(p, orow, n0_tile + c, av, gv);
     }
-  } else if ((EPI == EPI_BF16 || EPI == EPI_BF16_RELU || EPI == EPI_BF16_SILU || EPI == EPI_BF16_RELPOS) &&
+  } else if ((EPI == EPI_BF16 || EPI == EPI_BF16_RELU || EPI == EPI_BF16_SILU || EPI == EPI_BF16_RELPOS ||
+              EPI == EPI_BF16_GELU) &&
              p.bf16_coalesced) {
     // bf16 outputs: 64 accumulator columns (= 128 bytes per row) per round through the warp's staging tile, so a
     // warp store covers 4 rows x 128 contiguous bytes instead of 32 rows x 16 bytes (8x fewer LSU wavefronts)
@@ -567,6 +572,10 @@ __device__ __forceinline__ void drain_tile(const GemmKParams& p, const TileCoord
           if (EPI == EPI_BF16_RELU) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) v[e] = fmaxf(v[e], 0.f);
+          }
+          if (EPI == EPI_BF16_GELU) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) v[e] = gelu_erf(v[e]);
           }
           if constexpr (EPI == EPI_BF16_RELPOS) {
             if (kcols) {
@@ -1104,6 +1113,7 @@ static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
     case EPI_GLU: kern = pair ? gemm_wg_kernel<BN, EPI_GLU, true> : gemm_wg_kernel<BN, EPI_GLU, false>; break;
     case EPI_LSE: kern = gemm_wg_kernel<BN, EPI_LSE, false>; break;
     case EPI_BF16_RELPOS: kern = gemm_wg_kernel<BN, EPI_BF16_RELPOS, false>; break;
+    case EPI_BF16_GELU: kern = gemm_wg_kernel<BN, EPI_BF16_GELU, false>; break;
     default: kern = gemm_wg_kernel<BN, EPI_GENERIC, false>; break;
   }
   RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES));
@@ -1197,6 +1207,11 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
                     (reinterpret_cast<uintptr_t>(a.rp_v) & 15) == 0,
                 "gemm: rel-pos epilogue needs a plain bf16 output, 64-aligned key columns and 16-byte aligned tables");
     RVB_REQUIRE(get_gemm_impl() != 1, "gemm: rel-pos epilogue is not built for the simt bring-up kernel");
+  }
+  if (a.act == ACT_GELU) {
+    RVB_REQUIRE(a.out_mode == OUT_BF16 && a.out_split == 0 && !a.x3 && !a.grp && !a.rp_pos,
+                "gemm: ACT_GELU needs a plain bf16 output");
+    RVB_REQUIRE(get_gemm_impl() != 1, "gemm: ACT_GELU is not built for the simt bring-up kernel");
   }
   if (a.out_mode == OUT_LSE) {
     RVB_REQUIRE(a.lse_gather && a.lse_part && a.lse_tgt && a.act == ACT_NONE && !a.conv_mode && a.N > 128,

@@ -1,6 +1,8 @@
 // reverb_b200 — host-side launchers of the sm_90a kernels (internal; the public boundary is
 // include/rvb_b200.h).  Every launcher enqueues on the given stream and returns 0 / <0.
 #pragma once
+#include <vector>
+
 #include "common.cuh"
 
 struct rvb_model;
@@ -16,7 +18,8 @@ int search_side_stream(::rvb_model* m, cudaStream_t* out);
 // ACT_GLU (bf16 output only): the N = 2C weight rows are interleaved in groups of 32 — rows [64j, 64j+32) are the
 // "value" half of output channels [32j, 32j+32), rows [64j+32, 64j+64) their gates — and the kernel writes
 // out[m, 32j + i] = (acc_a + bias_a) * sigmoid(acc_g + bias_g), an (M, C) matrix (default ldo = N / 2).
-enum GemmAct { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_GLU = 3 };
+// ACT_GELU (bf16 output only): torch's default erf GELU, 0.5 x (1 + erf(x / sqrt 2)).
+enum GemmAct { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_GLU = 3, ACT_GELU = 4 };
 enum GemmOut {
   OUT_BF16 = 0,      // out_bf16[m, n] = act(acc + bias)
   OUT_F32 = 1,       // out_f32[m, n]  = act(acc + bias)
@@ -113,6 +116,22 @@ int launch_fbank_batch(const void* wave, int is_i16, int batch, long long wave_s
 // C[m, n] = act(sum_k A[m, k] W[n, k] + bias[n]) in fp32 on the CUDA cores; act 1 = LeakyReLU(0.01)
 int launch_sgemm(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc, int M, int N,
                  int K, int act, cudaStream_t stream);
+class WeightStore;
+// The head both segmentation networks share (PyanNet and WavLM / SSeRiouSS): bidirectional LSTM stack -> linears with
+// LeakyReLU -> classifier -> log_softmax, fp32, under pyannote's names lstm.*, linear.{i}.*, classifier.*.
+struct SegHead {
+  int hidden = 128, lstm_layers = 0, linear_layers = 0, linear_dim = 0, num_classes = 0;
+  std::vector<float*> wih, whh, lbias;   // per layer: (2*4H, in), (2, 4H, H), (2*4H)
+  std::vector<float*> lin_w, lin_b;
+  float* cls_w = nullptr;
+  float* cls_b = nullptr;
+};
+// uploads the head's tensors from the store (in_dim: width of the LSTM input); shape fields must be set
+int seg_head_load(WeightStore& store, int in_dim, SegHead* h);
+// x (B*T, in_dim) -> logp (B*T, classes).  Scratch: g (B*T, 8H), h0 / h1 (B*T, 2H) (x may be h1, not h0),
+// y0 / y1 (B*T, max(linear_dim, classes))
+int seg_head_forward(const SegHead& h, const float* x, int in_dim, int B, int T, float* g, float* h0, float* h1,
+                     float* y0, float* y1, float* logp, cudaStream_t stream);
 
 // ------------------------------------------------------------------ norms / conv pieces (elementwise.cu)
 // y = LN(x) * gamma + beta ; rows with position >= row_lens[batch] are written as 0 when mask_rows != 0.
@@ -197,6 +216,10 @@ struct AttnTcArgs {
   const uint32_t* key_bits = nullptr;
   int bits_ld = 0;
   float scale = 1.0f;
+  // WavLM's gated relative-position bias (self-attention, Tq == Tk, no other mask or key bias): score(i, j) +=
+  // gate[(group*H + h)*Tq + i] * rel_bias[h*(2Tk - 1) + j - i + Tk - 1], added after the scaling
+  const float* gate = nullptr;
+  const float* rel_bias = nullptr;
 };
 int launch_attention_tc(const AttnTcArgs& a, cudaStream_t stream);
 // CTAs per SM of the instantiation launch_attention_tc runs for these masks and Tk

@@ -4,7 +4,10 @@ CLI mirror of diarization/infer_pyannote3.0.py:16-42 (positional audios, --out-d
 --hf-access-token; output `<out-dir>/<basename>.rttm`).  Differences forced by the environment: there is no network, so
 `--pipeline-model` names a LOCAL directory holding `segmentation.pt` and `embedding.pt` (torch state_dicts under
 pyannote's key names, what `Model.from_pretrained(...).state_dict()` saves for the pipeline's two models) and the
-HuggingFace token is accepted and ignored; `--synthetic` runs seeded random weights (benchmarks, smoke tests).
+HuggingFace token is accepted and ignored; `--synthetic` runs seeded random weights of v1, `--synthetic-v2` of v2
+(benchmarks, smoke tests).
+A segmentation checkpoint whose keys start with `wav2vec.` is reverb-diarization-v2's WavLM model, any other PyanNet
+(v1).  Both use the pyannote 3.1 pipeline hyper-parameters (v2's own are not available offline).
 """
 from __future__ import annotations
 
@@ -19,7 +22,7 @@ import torch
 from . import synth
 from .embedding import EmbeddingModel
 from .pipeline import SpeakerDiarization
-from .segmentation import SegmentationModel
+from .segmentation import segmentation_model
 
 
 def _load_state_dict(path: str) -> Dict[str, np.ndarray]:
@@ -29,16 +32,20 @@ def _load_state_dict(path: str) -> Dict[str, np.ndarray]:
     return {k: v.float().numpy() for k, v in sd.items() if torch.is_tensor(v) and v.is_floating_point()}
 
 
-def load_pipeline(model_dir: str = None, synthetic: bool = False, device: int = 0, **kwargs) -> SpeakerDiarization:
+def load_pipeline(model_dir: str = None, synthetic=False, device: int = 0, **kwargs) -> SpeakerDiarization:
+    """synthetic: False (load `model_dir`), True or "v1" (seeded PyanNet weights), "v2" (seeded WavLM weights)."""
+    if synthetic not in (False, None, True, "v1", "v2"):
+        raise ValueError(f"synthetic must be 'v1' or 'v2', not {synthetic!r}")
     if synthetic:
-        seg_sd, emb_sd = synth.segmentation_state_dict(0), synth.embedding_state_dict(0)
+        seg_sd = (synth.wavlm_segmentation_state_dict(0) if synthetic == "v2" else synth.segmentation_state_dict(0))
+        emb_sd = synth.embedding_state_dict(0)
     else:
         if not model_dir or not os.path.isdir(model_dir):
             raise ValueError(f"pipeline model directory {model_dir!r} not found (no network: pass a local directory with "
                              "segmentation.pt and embedding.pt, or --synthetic)")
         seg_sd = _load_state_dict(os.path.join(model_dir, "segmentation.pt"))
         emb_sd = _load_state_dict(os.path.join(model_dir, "embedding.pt"))
-    return SpeakerDiarization(SegmentationModel(seg_sd, device=device), EmbeddingModel(emb_sd, device=device), **kwargs)
+    return SpeakerDiarization(segmentation_model(seg_sd, device=device), EmbeddingModel(emb_sd, device=device), **kwargs)
 
 
 def read_audio(path: str) -> np.ndarray:
@@ -70,10 +77,13 @@ def main(argv=None) -> int:
     ap.add_argument("--out-dir", type=Path, required=True)
     ap.add_argument("--hf-access-token", type=str, default=None, help="accepted for CLI compatibility; unused offline")
     ap.add_argument("--pipeline-model", type=str, default=None, help="local directory with segmentation.pt / embedding.pt")
-    ap.add_argument("--synthetic", action="store_true", help="seeded random weights (no checkpoint available offline)")
+    syn = ap.add_mutually_exclusive_group()
+    syn.add_argument("--synthetic", action="store_true", help="seeded random weights (no checkpoint available offline)")
+    syn.add_argument("--synthetic-v2", action="store_true",
+                     help="seeded random weights of reverb-diarization-v2 (WavLM segmentation)")
     args = ap.parse_args(argv)
     os.makedirs(args.out_dir, exist_ok=True)
-    pipe = load_pipeline(args.pipeline_model, synthetic=args.synthetic)
+    pipe = load_pipeline(args.pipeline_model, synthetic="v2" if args.synthetic_v2 else args.synthetic)
     for audio in args.audios:
         print("Processing", audio)
         turns = pipe(read_audio(audio))

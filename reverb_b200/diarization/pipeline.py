@@ -250,7 +250,10 @@ class SpeakerDiarization:
         self.seg_batch_size = segmentation_batch_size or max(batch_size, 264)
         self.embedding_min_samples = embedding_min_samples
         self.mapping = powerset_mapping(max_speakers_per_chunk, max_speakers_per_frame)
-        self.frames = receptive_field(sample_rate)
+        # the segmentation model's own frame grid when it declares one (WavLM: 400 / 320 samples), else PyanNet's
+        rf = getattr(segmentation, "receptive_field", None)
+        self.frames = (SlidingWindow(0.0, rf[0] / sample_rate, rf[1] / sample_rate) if rf is not None
+                       else receptive_field(sample_rate))
 
     # -- stage 1: local segmentation of every window (`get_segmentations` + hard powerset conversion) -----------------
     def windows(self, wave: torch.Tensor) -> torch.Tensor:

@@ -48,10 +48,16 @@ def segmentation_state_dict(seed: int = 0, shape: Dict = SEG_SHAPE) -> Dict[str,
         bound = 1.0 / math.sqrt(cin * k)
         sd[f"sincnet.conv1d.{i}.weight"] = _uniform(rng, (shape["conv_channels"], cin, k), bound)
         sd[f"sincnet.conv1d.{i}.bias"] = _uniform(rng, (shape["conv_channels"],), bound)
+    _head_state_dict(rng, sd, shape["conv_channels"], shape)
+    return sd
+
+
+def _head_state_dict(rng, sd: Dict[str, np.ndarray], in_dim: int, shape: Dict) -> None:
+    """PyanNet's head (LSTM, linears, classifier) on `in_dim` input features, drawn from `rng` in that order."""
     H = shape["lstm_hidden"]
     bound = 1.0 / math.sqrt(H)
     for layer in range(shape["lstm_layers"]):
-        cin = shape["conv_channels"] if layer == 0 else 2 * H
+        cin = in_dim if layer == 0 else 2 * H
         for sfx in ("", "_reverse"):
             # larger than PyTorch's default so that the random network reacts to its input (default-init LSTMs are flat)
             sd[f"lstm.weight_ih_l{layer}{sfx}"] = _uniform(rng, (4 * H, cin), 4.0 * bound)
@@ -67,6 +73,63 @@ def segmentation_state_dict(seed: int = 0, shape: Dict = SEG_SHAPE) -> Dict[str,
     bound = 6.0 / math.sqrt(cin)
     sd["classifier.weight"] = _uniform(rng, (shape["num_classes"], cin), bound)
     sd["classifier.bias"] = _uniform(rng, (shape["num_classes"],), 0.5)
+
+
+# reverb-diarization-v2: pyannote SSeRiouSS on torchaudio's wavlm_base(), PyanNet's head
+WAVLM_SEG_SHAPE = dict(sample_rate=16000, conv_channels=512, embed_dim=768, num_layers=12, num_heads=12, ffn_dim=3072,
+                       pos_conv_kernel=128, pos_conv_groups=16, num_buckets=320, max_distance=800, lstm_hidden=128,
+                       lstm_layers=4, linear_dim=128, linear_layers=2, num_classes=7)
+WAVLM_CONV = ((10, 5), (3, 2), (3, 2), (3, 2), (3, 2), (2, 2), (2, 2))   # (kernel, stride) of the feature extractor
+
+
+def wavlm_segmentation_state_dict(seed: int = 0, shape: Dict = WAVLM_SEG_SHAPE) -> Dict[str, np.ndarray]:
+    """SSeRiouSS weights under pyannote's names (`wav2vec.` + torchaudio's wavlm_base names, `wav2vec_weights`, the
+    head's): PyTorch-default uniform initialisation, norms and gates away from the identity so that every term is
+    exercised."""
+    rng = np.random.default_rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    C, D, H, F = shape["conv_channels"], shape["embed_dim"], shape["num_heads"], shape["ffn_dim"]
+    p = "wav2vec."
+    fe = p + "feature_extractor.conv_layers."
+    cin = 1
+    for i, (k, _) in enumerate(WAVLM_CONV):
+        sd[f"{fe}{i}.conv.weight"] = _uniform(rng, (C, cin, k), math.sqrt(3.0 / (cin * k)))
+        cin = C
+    sd[fe + "0.layer_norm.weight"] = rng.uniform(0.8, 1.2, C).astype(np.float32)
+    sd[fe + "0.layer_norm.bias"] = rng.uniform(-0.1, 0.1, C).astype(np.float32)
+    fp = p + "encoder.feature_projection."
+    sd[fp + "layer_norm.weight"] = rng.uniform(0.8, 1.2, C).astype(np.float32)
+    sd[fp + "layer_norm.bias"] = rng.uniform(-0.1, 0.1, C).astype(np.float32)
+    sd[fp + "projection.weight"] = _uniform(rng, (D, C), 1.0 / math.sqrt(C))
+    sd[fp + "projection.bias"] = _uniform(rng, (D,), 1.0 / math.sqrt(C))
+    K, G = shape["pos_conv_kernel"], shape["pos_conv_groups"]
+    pc = p + "encoder.transformer.pos_conv_embed.conv."
+    sd[pc + "bias"] = _uniform(rng, (D,), 0.1)
+    sd[pc + "parametrizations.weight.original0"] = rng.uniform(0.5, 1.5, (1, 1, K)).astype(np.float32)
+    sd[pc + "parametrizations.weight.original1"] = rng.normal(0, 1, (D, D // G, K)).astype(np.float32)
+    sd[p + "encoder.transformer.layer_norm.weight"] = rng.uniform(0.8, 1.2, D).astype(np.float32)
+    sd[p + "encoder.transformer.layer_norm.bias"] = rng.uniform(-0.1, 0.1, D).astype(np.float32)
+    for l in range(shape["num_layers"]):
+        q = f"{p}encoder.transformer.layers.{l}."
+        if l == 0:
+            sd[q + "attention.rel_attn_embed.weight"] = rng.normal(0, 1, (shape["num_buckets"], H)).astype(np.float32)
+        b = 1.0 / math.sqrt(D)
+        sd[q + "attention.attention.in_proj_weight"] = _uniform(rng, (3 * D, D), math.sqrt(3.0) * b)
+        sd[q + "attention.attention.in_proj_bias"] = _uniform(rng, (3 * D,), b)
+        sd[q + "attention.attention.out_proj.weight"] = _uniform(rng, (D, D), b)
+        sd[q + "attention.attention.out_proj.bias"] = _uniform(rng, (D,), b)
+        sd[q + "attention.gru_rel_pos_const"] = rng.uniform(0.5, 1.5, (1, H, 1, 1)).astype(np.float32)
+        sd[q + "attention.gru_rel_pos_linear.weight"] = _uniform(rng, (8, D // H), 1.0 / math.sqrt(D // H))
+        sd[q + "attention.gru_rel_pos_linear.bias"] = _uniform(rng, (8,), 1.0 / math.sqrt(D // H))
+        for n in ("layer_norm", "final_layer_norm"):
+            sd[q + n + ".weight"] = rng.uniform(0.8, 1.2, D).astype(np.float32)
+            sd[q + n + ".bias"] = rng.uniform(-0.1, 0.1, D).astype(np.float32)
+        sd[q + "feed_forward.intermediate_dense.weight"] = _uniform(rng, (F, D), b)
+        sd[q + "feed_forward.intermediate_dense.bias"] = _uniform(rng, (F,), b)
+        sd[q + "feed_forward.output_dense.weight"] = _uniform(rng, (D, F), 1.0 / math.sqrt(F))
+        sd[q + "feed_forward.output_dense.bias"] = _uniform(rng, (D,), 1.0 / math.sqrt(F))
+    sd["wav2vec_weights"] = rng.uniform(-1.0, 1.0, shape["num_layers"]).astype(np.float32)
+    _head_state_dict(rng, sd, D, shape)
     return sd
 
 

@@ -63,6 +63,8 @@ def get_args(argv=None):
                         "write <result_dir>/<mode>/<stem>.stm and <result_dir>/rttm/<stem>.rttm")
     p.add_argument("--diarization_synthetic", action="store_true",
                    help="Like --diarization_model, with the seeded synthetic diarization weights")
+    p.add_argument("--diarization_synthetic_v2", action="store_true",
+                   help="Like --diarization_synthetic, with reverb-diarization-v2's (WavLM segmentation)")
     p.add_argument("--log_level", choices=["DEBUG", "INFO", "WARNING", "ERROR", "CRITICAL"], default="INFO")
     args = p.parse_args(argv)
     if isinstance(args.verbatimicity, list):           # one value stays a float; else one per --audio_file
@@ -105,9 +107,10 @@ def main(argv=None):
         out_dirs.append(Path(args.result_dir) / mode)
         os.makedirs(out_dirs[-1], exist_ok=True)
     diarization = None
-    if args.diarization_model or args.diarization_synthetic:
+    if args.diarization_model or args.diarization_synthetic or args.diarization_synthetic_v2:
         from .diarization.infer import load_pipeline
-        diarization = load_pipeline(args.diarization_model, synthetic=args.diarization_synthetic)
+        diarization = load_pipeline(args.diarization_model,
+                                    synthetic="v2" if args.diarization_synthetic_v2 else args.diarization_synthetic)
         os.makedirs(Path(args.result_dir) / "rttm", exist_ok=True)
     graph = asr.context_graph(args.context_list_path, args.context_graph_score) if args.context_list_path else None
     results = asr.transcribe_files(
