@@ -177,7 +177,8 @@ RVB_API int rvb_attention_rescoring(rvb_model* m, const float* d_enc_out, const 
 /* ctc_prefix_beam_search + attention_rescoring in one call, the n-best staying on the device in between
  * (what ASRModel.decode does for method "attention_rescoring", asr_model.py:259-308 / search.py:124-248,378-444).
  * Host outputs are written COMPACT with row length L = *out_max_len (the longest hypothesis / times list, >= 1):
- * h_tokens / h_times (B, beam, L), h_l2r / h_r2l (B, beam, L + 1); the caller provides room for L = cap.
+ * h_tokens / h_times (B, beam, L), 0 past each row's n_tokens / n_times, h_l2r / h_r2l (B, beam, L + 1); the caller
+ * provides room for L = cap.
  * h_lens (B, beam, 2) = {n_tokens, n_times}, h_scores (B, beam) float64 CTC scores, h_nhyp (B).
  * h_r2l may be NULL (or reverse_weight == 0): the right-to-left decoder is skipped. */
 RVB_API int rvb_beam_search_rescoring(rvb_model* m, const float* d_topk_val, const int* d_topk_idx, int k,

@@ -61,7 +61,6 @@ struct EncLayer {
   bool lsl = false;
   int lsl_idx = -1;                    // index among the encoder's LSL layers (LangStack)
   std::vector<float*> lang_w, lang_b;  // fp32 device copies of language_layers.{i}
-  Linear lang;                         // folded with the current cat_embs
 };
 
 struct DecLayer {
@@ -71,23 +70,22 @@ struct DecLayer {
   bool lsl = false;
   int lsl_idx = -1;  // index among the LSL layers of both decoders (LangStack)
   std::vector<float*> lang_w, lang_b;
-  Linear lang;
 };
 
 struct SearchTicket;
 struct DecCache;
 
-// The folds of the G distinct mixing vectors of a per-utterance cat_embs, side by side for every LSL layer of the
-// encoder (or of the decoders): weight (G*d, d) — the (G*d, 2d) pair layout in the accurate mode — and bias (G*d),
-// grow-only, read by the grouped LSL GEMM (GemmArgs::grp).  `key` holds the vectors they were folded for, in group
-// order: a batch with the same ordered set folds nothing.
+// The folds of the distinct mixing vectors of a call, slot g for its group g, side by side for every LSL layer of the
+// encoder (or of the decoders): weight (slots*d, d) — the (slots*d, 2d) pair layout in the accurate mode — and bias
+// (slots*d), grow-only and sized exactly, slots = key.size().  key[g] is the vector slot g holds (empty: none), so a
+// slot refolds only when its vector changes; growing reallocates the buffers and so empties every key.
 struct LangStack {
-  std::vector<DevBuf> w, b;  // by lsl_idx
-  std::vector<float> key;
+  std::vector<DevBuf> w, b;             // by lsl_idx
+  std::vector<std::vector<float>> key;  // by slot
 };
 
-// The language-specific mixing of one call's utterances: uniform (G == 0: the layers' folded Linear), or G groups
-// with each utterance's group id on the device (owned by the call, its ticket or its decoder cache) and
+// The language-specific mixing of one call's utterances: one vector (G == 0: plain launches of slot 0 of st), or G
+// groups with each utterance's group id on the device (owned by the call, its ticket or its decoder cache) and
 // rows_per_batch GEMM rows per utterance.
 struct CatRows {
   int G = 0;
@@ -162,8 +160,8 @@ struct NBest {
   }
 };
 
-// The packed weights of a plan, uploaded by rvb_model_finalize into the plan's WeightStore.  A fork copies them and
-// replaces only the folded language-specific linears (EncLayer::lang, DecLayer::lang) by its own.
+// The packed weights of a plan, uploaded by rvb_model_finalize into the plan's WeightStore and never written after it:
+// a fork copies them as they are.
 struct Weights {
   float* cmvn_mean = nullptr;
   float* cmvn_istd = nullptr;
@@ -187,8 +185,7 @@ struct rvb_model {
   WeightStore store{"model:"};  // raw reference tensors until finalize, and the device allocations of this plan
   bool finalized = false;
   Weights w;
-  std::vector<float> cur_cat;  // cat_embs the LSL folds were computed for
-  rvb::LangStack st_enc, st_dec;  // stacked folds of per-utterance cat_embs (encoder, decoders)
+  rvb::LangStack st_enc, st_dec;  // folds of the calls' cat_embs (encoder, decoders)
   DevBuf ws_grp;                  // group ids of attention_rescoring, which waits for its stream before it returns
   HostPinned pin_grp;
   bool x3 = false;             // cfg.precision == 1: bf16x3 "fp32-accurate" mode (GemmArgs::x3, kernels.h)
@@ -314,17 +311,8 @@ static int load_fused(rvb_model* m, const std::string& prefix, const std::vector
   return 0;
 }
 
-// zeroed device space of a language-specific linear that fold_lang fills for the current cat_embs
-static int alloc_fold(rvb_model* m, Linear* folded) {
-  const int d = m->cfg.d_model;
-  if (m->store.alloc_zeroed((size_t)d * d * m->pm(), &folded->w) || m->store.alloc_zeroed(d, &folded->b)) return -1;
-  folded->N = d;
-  folded->K = d;
-  return 0;
-}
-
 static int load_lang(rvb_model* m, const std::string& prefix, int d, int n_lang, std::vector<float*>* lw,
-                     std::vector<float*>* lb, Linear* folded) {
+                     std::vector<float*>* lb) {
   for (int i = 0; i < n_lang; ++i) {
     const std::vector<float>*w, *b;
     std::string p = prefix + ".language_layers." + std::to_string(i);
@@ -334,7 +322,7 @@ static int load_lang(rvb_model* m, const std::string& prefix, int d, int n_lang,
     lw->push_back(dw);
     lb->push_back(db);
   }
-  return alloc_fold(m, folded);
+  return 0;
 }
 
 static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Decoder* dec, int* n_lsl) {
@@ -362,7 +350,7 @@ static int load_decoder(rvb_model* m, const std::string& side, int nblocks, Deco
     if (load_linear(m, q + ".src_attn.linear_out", d, d, &L.co)) return -1;
     if (load_linear(m, q + ".feed_forward.w_1", c.dec_ffn_dim, d, &L.ff1)) return -1;
     if (load_linear(m, q + ".feed_forward.w_2", d, c.dec_ffn_dim, &L.ff2)) return -1;
-    if (L.lsl && load_lang(m, q, d, c.num_langs, &L.lang_w, &L.lang_b, &L.lang)) return -1;
+    if (L.lsl && load_lang(m, q, d, c.num_langs, &L.lang_w, &L.lang_b)) return -1;
     if (L.lsl) L.lsl_idx = (*n_lsl)++;
   }
   dec->present = true;
@@ -445,7 +433,7 @@ static int finalize_model(rvb_model* m) {
       if (m->store.need(p + ".conv_module.norm.running_var", d, &t) || m->store.upload(t->data(), d, &E.bn_var))
         return -1;
     }
-    if (E.lsl && load_lang(m, p, d, c.num_langs, &E.lang_w, &E.lang_b, &E.lang)) return -1;
+    if (E.lsl && load_lang(m, p, d, c.num_langs, &E.lang_w, &E.lang_b)) return -1;
     if (E.lsl) E.lsl_idx = i == 0 ? 0 : 1;
   }
   if (upload_w(m, posw.data(), (size_t)L * d, d, &m->w.pos_all.w)) return -1;
@@ -461,33 +449,6 @@ static int finalize_model(rvb_model* m) {
   }
   m->store.drop_host();
   m->finalized = true;
-  return 0;
-}
-
-// fold sum_i c_i * language_layers[i] for every LSL layer (encoder_layer.py:376-390, decoder_layer.py:318-331)
-static int fold_lang(rvb_model* m, const float* cat, int n_cat, cudaStream_t stream) {
-  const rvb_model_config& c = m->cfg;
-  if (c.num_langs == 0) return 0;
-  RVB_REQUIRE(cat != nullptr && n_cat == c.num_langs, "cat_embs of length %d required (got %d)", c.num_langs, n_cat);
-  if ((int)m->cur_cat.size() == n_cat && memcmp(m->cur_cat.data(), cat, sizeof(float) * n_cat) == 0) return 0;
-  const int d = c.d_model;
-  if (m->x3 && m->ws_fold.ensure((size_t)d * d * sizeof(float))) return -1;
-  auto fold = [&](std::vector<float*>& lw, std::vector<float*>& lb, Linear& out) -> int {
-    if (m->x3) {  // fold in fp32, then split into the (d, 2d) hi/lo pair
-      float* tmp = m->ws_fold.as<float>();
-      if (launch_weighted_sum_bf16(lw.data(), cat, n_cat, (long long)d * d, nullptr, tmp, stream)) return -1;
-      if (launch_f32_to_pair(tmp, out.w, d, d, stream)) return -1;
-    } else if (launch_weighted_sum_bf16(lw.data(), cat, n_cat, (long long)d * d, out.w, nullptr, stream)) return -1;
-    if (launch_weighted_sum_bf16(lb.data(), cat, n_cat, d, nullptr, out.b, stream)) return -1;
-    return 0;
-  };
-  for (auto& E : m->w.enc)
-    if (E.lsl && fold(E.lang_w, E.lang_b, E.lang)) return -1;
-  for (Decoder* D : {&m->w.dec_l, &m->w.dec_r})
-    if (D->present)
-      for (auto& Ld : D->layers)
-        if (Ld.lsl && fold(Ld.lang_w, Ld.lang_b, Ld.lang)) return -1;
-  m->cur_cat.assign(cat, cat + n_cat);
   return 0;
 }
 
@@ -513,26 +474,35 @@ static int group_cat(const rvb_model* m, const float* cat, int n_cat, int B, std
   return 0;
 }
 
-// fold each of the G vectors of `cat` (G * num_langs) the way fold_lang folds one, into the stacked folds of the
-// encoder's (dec = false) or the decoders' LSL layers, on the stream of the kernels that read them
+// fold sum_i c_i * language_layers[i] (encoder_layer.py:376-390, decoder_layer.py:318-331) of each of the G vectors of
+// `cat` (G * num_langs) into slot g of the stack of the encoder's (dec = false) or the decoders' LSL layers, on the
+// stream of the kernels that read them.  A slot that holds its vector already folds nothing.
 static int fold_stack(rvb_model* m, bool dec, const std::vector<float>& cat, cudaStream_t stream) {
+  const int d = m->cfg.d_model, L = m->cfg.num_langs;
+  if (L == 0) return 0;
   LangStack& st = dec ? m->st_dec : m->st_enc;
-  if (st.key.size() == cat.size() && memcmp(st.key.data(), cat.data(), sizeof(float) * cat.size()) == 0) return 0;
-  st.key.clear();
-  const int d = m->cfg.d_model, L = m->cfg.num_langs, G = (int)cat.size() / L;
-  const size_t pm = (size_t)m->pm();
+  const int G = (int)cat.size() / L;
+  if (G > (int)st.key.size()) st.key.assign(G, {});  // the buffers (key.size() slots, exactly) grow below
+  std::vector<int> stale;
+  for (int g = 0; g < G; ++g)
+    if (st.key[g].size() != (size_t)L || memcmp(st.key[g].data(), &cat[(size_t)g * L], sizeof(float) * L) != 0) {
+      st.key[g].clear();
+      stale.push_back(g);
+    }
+  if (stale.empty()) return 0;
+  const size_t pm = (size_t)m->pm(), slots = st.key.size();
   if (m->x3 && m->ws_fold.ensure((size_t)d * d * sizeof(float))) return -1;
   auto fold = [&](std::vector<float*>& lw, std::vector<float*>& lb, int idx) -> int {
     if ((int)st.w.size() <= idx) {
       st.w.resize(idx + 1);
       st.b.resize(idx + 1);
     }
-    if (st.w[idx].ensure((size_t)G * d * d * pm * sizeof(bf16)) || st.b[idx].ensure((size_t)G * d * sizeof(float)))
+    if (st.w[idx].ensure(slots * d * d * pm * sizeof(bf16), true) || st.b[idx].ensure(slots * d * sizeof(float), true))
       return -1;
-    for (int g = 0; g < G; ++g) {
+    for (int g : stale) {
       const float* c = cat.data() + (size_t)g * L;
       bf16* w = st.w[idx].as<bf16>() + (size_t)g * d * d * pm;
-      if (m->x3) {
+      if (m->x3) {  // fold in fp32, then split into the (d, 2d) hi/lo pair
         float* tmp = m->ws_fold.as<float>();
         if (launch_weighted_sum_bf16(lw.data(), c, L, (long long)d * d, nullptr, tmp, stream)) return -1;
         if (launch_f32_to_pair(tmp, w, d, d, stream)) return -1;
@@ -550,23 +520,22 @@ static int fold_stack(rvb_model* m, bool dec, const std::vector<float>& cat, cud
         for (auto& Ld : D->layers)
           if (Ld.lsl && fold(Ld.lang_w, Ld.lang_b, Ld.lsl_idx)) return -1;
   }
-  st.key = cat;
+  for (int g : stale) st.key[g].assign(&cat[(size_t)g * L], &cat[(size_t)g * L] + L);
   return 0;
 }
 
-// The one place that chooses between the uniform and the grouped LSL path of a call: one distinct vector (cat_embs of
-// num_langs, or B rows with equal bits) runs fold_lang and the plain launches; G > 1 distinct vectors fold the stack of
-// the encoder (dec = false) or of the decoders.  -> *G (0 = uniform), uniq (the vectors), grp (each utterance's group).
-static int prepare_cat(rvb_model* m, bool dec, const float* cat, int n_cat, int B, std::vector<float>* uniq,
-                       std::vector<int>* grp, int* G, cudaStream_t stream) {
-  if (group_cat(m, cat, n_cat, B, uniq, grp)) return -1;
-  const int L = m->cfg.num_langs;
-  *G = L ? (int)uniq->size() / L : 0;
-  if (*G <= 1) {
-    *G = 0;
-    return L ? fold_lang(m, uniq->data(), L, stream) : 0;
-  }
-  return fold_stack(m, dec, *uniq, stream);
+// The LSL mixing of one call over B utterances: the distinct vectors of its cat_embs (group_cat) folded into the stack
+// of the encoder (dec = false) or of the decoders; G = 0 when there is one.  -> grp, each utterance's group, for the
+// caller to upload where the call's lifetime requires (cr->d_grp, read when G > 1), and the vectors in uniq if asked.
+static int cat_rows(rvb_model* m, bool dec, const float* cat, int n_cat, int B, CatRows* cr, std::vector<int>* grp,
+                    cudaStream_t stream, std::vector<float>* uniq = nullptr) {
+  std::vector<float> own;
+  if (uniq == nullptr) uniq = &own;
+  if (group_cat(m, cat, n_cat, B, uniq, grp) || fold_stack(m, dec, *uniq, stream)) return -1;
+  const int L = m->cfg.num_langs, G = L ? (int)uniq->size() / L : 0;
+  cr->G = G > 1 ? G : 0;
+  cr->st = dec ? &m->st_dec : &m->st_enc;
+  return 0;
 }
 
 // B group ids -> dev through the page-locked pin, on `stream`
@@ -603,21 +572,22 @@ static int gemm(rvb_model* m, const bf16* A, const Linear& W, int M, int act, in
   return launch_gemm(g, stream);
 }
 
-// The language-specific linear of one LSL layer over M rows: the uniformly folded weight `uni`, or one grouped launch
-// over the stacked folds (layer lsl_idx of cr.st), every row taking its utterance's fold
-static int lang_gemm(rvb_model* m, const bf16* A, const Linear& uni, int lsl_idx, const CatRows& cr, int M, int out_mode,
-                     void* out, cudaStream_t stream) {
-  if (cr.G == 0) return gemm(m, A, uni, M, ACT_NONE, out_mode, out, 1.f, stream);
+// The language-specific linear of one LSL layer over M rows, from the folds of layer lsl_idx of cr.st: a plain launch
+// of slot 0 for one vector (cr.G == 0), else one grouped launch, every row taking its utterance's slot
+static int lang_gemm(rvb_model* m, const bf16* A, int lsl_idx, const CatRows& cr, int M, int out_mode, void* out,
+                     cudaStream_t stream) {
   const int d = m->cfg.d_model;
+  const Linear slot0{cr.st->w[lsl_idx].as<bf16>(), cr.st->b[lsl_idx].as<float>(), d, d};
+  if (cr.G == 0) return gemm(m, A, slot0, M, ACT_NONE, out_mode, out, 1.f, stream);
   GemmArgs g;
   g.x3 = m->x3 ? 1 : 0;
   if (m->x3 && out_mode == OUT_BF16) g.out_split = d;
   g.A = A;
-  g.W = cr.st->w[lsl_idx].as<bf16>();
+  g.W = slot0.w;
   g.M = M;
   g.N = cr.G * d;
   g.K = d;
-  g.bias = cr.st->b[lsl_idx].as<float>();
+  g.bias = slot0.b;
   g.act = ACT_NONE;
   g.out_mode = out_mode;
   g.out = out;
@@ -733,10 +703,9 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
   const int T1h = (T1 + 1) / 2;
   const long long M = (long long)B * Tp;
   RVB_REQUIRE(M * (long long)F2 < (1ll << 31), "encoder_forward: batch too large (B*T'*F2 overflows int)");
-  std::vector<float> cat_u;
   std::vector<int> grp;
   CatRows cr;
-  if (prepare_cat(m, false, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+  if (cat_rows(m, false, h_cat, n_cat, B, &cr, &grp, stream)) return -1;
 
   // lengths
   // pinned staging ring: a back-to-back call must not overwrite lengths an earlier async copy still reads.  Slots are
@@ -760,7 +729,6 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
   RVB_CHECK_CUDA(cudaMemcpyAsync(d_lens, h_lens, sizeof(int) * (cr.G ? m->lens_cap + B : B), cudaMemcpyHostToDevice,
                                  stream));
   cr.d_grp = d_lens + m->lens_cap;
-  cr.st = &m->st_enc;
   cr.rows_per_batch = Tp;
 
   // workspace
@@ -976,7 +944,7 @@ static int encoder_forward(rvb_model* m, const float* d_feats, const int* h_feat
     if (launch_layernorm(x, E.norm_ff.g, E.norm_ff.b, 1e-5f, (int)M, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
     const bf16* ffn_in = n;
     if (E.lsl) {
-      if (lang_gemm(m, n, E.lang, E.lsl_idx, cr, (int)M, OUT_F32, y, stream)) return -1;
+      if (lang_gemm(m, n, E.lsl_idx, cr, (int)M, OUT_F32, y, stream)) return -1;
       if (x3 ? launch_f32_to_pair(y, ybf, M, d, stream) : launch_f32_to_bf16(y, ybf, M * d, stream)) return -1;
       ffn_in = ybf;
     }
@@ -1055,7 +1023,7 @@ static int decoder_layers(rvb_model* m, Decoder& D, DecRows& w, int R, const Cat
     if (launch_layernorm(x, Ld.n3.g, Ld.n3.b, Ld.eps, R, d, n, nullptr, nullptr, 0, 0, stream, x3)) return -1;
     const bf16* ffn_in = n;
     if (Ld.lsl) {
-      if (lang_gemm(m, n, Ld.lang, Ld.lsl_idx, cr, R, OUT_BF16, ybf, stream)) return -1;
+      if (lang_gemm(m, n, Ld.lsl_idx, cr, R, OUT_BF16, ybf, stream)) return -1;
       ffn_in = ybf;
     }
     if (gemm(m, ffn_in, Ld.ff1, R, ACT_RELU, OUT_BF16, h, 1.f, stream)) return -1;
@@ -1183,10 +1151,9 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   RVB_REQUIRE(L >= 1 && k >= 1 && k <= 16 && k <= c.vocab, "decoder_step_topk: bad L=%d / k=%d", L, k);
   const int S = B * N;
   const long long R = (long long)S * L, Mem = (long long)B * Tp;
-  std::vector<float> cat_u;
   std::vector<int> grp;
   CatRows cr;
-  if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+  if (cat_rows(m, true, h_cat, n_cat, B, &cr, &grp, stream)) return -1;
   const size_t ints = (size_t)R + S + 2 * B;   // tokens | lengths | encoder lengths | LSL groups
   const size_t out_bytes = (size_t)S * k * (sizeof(float) + sizeof(int));
   const size_t row_bytes = h_logp ? (size_t)S * c.vocab * sizeof(float) : 0;
@@ -1203,7 +1170,6 @@ static int decoder_step_topk(rvb_model* m, const float* d_enc_out, const int* h_
   for (int b = 0; b < B; ++b) hp[R + S + B + b] = grp[b];
   int* dp = m->ws_misc.as<int>();
   cr.d_grp = dp + R + S + B;
-  cr.st = &m->st_dec;
   RVB_CHECK_CUDA(cudaMemcpyAsync(dp, hp, ints * sizeof(int), cudaMemcpyHostToDevice, stream));
   float* d_val = reinterpret_cast<float*>(dp + ints);
   int* d_idx = reinterpret_cast<int*>(d_val + (size_t)S * k);
@@ -1240,7 +1206,7 @@ struct DecCache {
   DevBuf logits, outv;
   HostPinned pin;
   std::vector<float> cat;  // the distinct LSL mixing vectors of decoder_cache_begin, refolded (if need be) every step
-  int G = 0;               // CatRows::G of the cached utterances, their groups in grp
+  CatRows cr;              // their mixing of the cached utterances, the groups in grp
   DevBuf grp;
   HostPinned grp_pin;
 };
@@ -1257,8 +1223,10 @@ static int decoder_cache_begin(rvb_model* m, const float* d_enc_out, const int* 
   const size_t pm = (size_t)m->pm(), nl = D.layers.size();
   const long long Mem = (long long)B * Tp;
   std::vector<int> grp;
-  if (prepare_cat(m, true, h_cat, n_cat, B, &dc.cat, &grp, &dc.G, stream)) return -1;
-  if (dc.G && upload_groups(grp, dc.grp_pin, dc.grp, stream)) return -1;
+  if (cat_rows(m, true, h_cat, n_cat, B, &dc.cr, &grp, stream, &dc.cat)) return -1;
+  if (dc.cr.G && upload_groups(grp, dc.grp_pin, dc.grp, stream)) return -1;
+  dc.cr.d_grp = dc.grp.as<int>();
+  dc.cr.rows_per_batch = N;
   dc.B = B; dc.Tp = Tp; dc.N = N; dc.S = S; dc.Lcap = Lcap; dc.step = 0; dc.flip = false;
   dc.self_a.resize(nl); dc.self_b.resize(nl); dc.cross.resize(nl);
   const size_t kvw = (size_t)2 * d * pm;  // cache row: [k | v] (x2 for the hi / lo pair layout)
@@ -1311,13 +1279,8 @@ static int decoder_cache_step(rvb_model* m, const int* h_tokens, const int* h_pa
   std::vector<DevBuf>& cur = dc.flip ? dc.self_b : dc.self_a;
   std::vector<DevBuf>& nxt = dc.flip ? dc.self_a : dc.self_b;
   const bool reorder = h_parents != nullptr && pos > 0;
-  CatRows cr;   // the folds of decoder_cache_begin's vectors: a call in between may have folded others
-  cr.G = dc.G;
-  cr.d_grp = dc.grp.as<int>();
-  cr.st = &m->st_dec;
-  cr.rows_per_batch = N;
-  if (c.num_langs && (dc.G ? fold_stack(m, true, dc.cat, stream) : fold_lang(m, dc.cat.data(), c.num_langs, stream)))
-    return -1;
+  if (fold_stack(m, true, dc.cat, stream)) return -1;  // a call in between may have folded other vectors
+  const CatRows& cr = dc.cr;
   bf16* qkv = dc.rows.qkv.as<bf16>();
   bf16* att = dc.rows.att.as<bf16>();
   if (launch_embed_posenc(d_tok, D.emb, S, 1, d, dc.rows.x.as<float>(), stream, pos)) return -1;
@@ -1491,13 +1454,11 @@ static int attention_rescoring(rvb_model* m, const float* d_enc_out, const int* 
   const int Lp = max_len + 1, S = B * N;
   const long long R = (long long)S * Lp;
   const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
-  std::vector<float> cat_u;
   std::vector<int> grp;
   CatRows cr;
-  if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+  if (cat_rows(m, true, h_cat, n_cat, B, &cr, &grp, stream)) return -1;
   if (cr.G && upload_groups(grp, m->pin_grp, m->ws_grp, stream)) return -1;
   cr.d_grp = m->ws_grp.as<int>();
-  cr.st = &m->st_dec;
   // the caller's hypotheses as an n-best with every slot present: an absent row (length < 0) is an empty hypothesis
   NBest& nb = m->nbest_in;
   const size_t rints = (size_t)R * 4 + S;
@@ -1582,12 +1543,14 @@ int search_side_stream(rvb_model* m, cudaStream_t* out) {
   return 0;
 }
 
-// The CTC prefix beam search into nb (rows of nb.len_cap tokens) on `stream`, with workspace ws: uploads the encoder
-// lengths through nb's host mirror, then searches, context-biased when graph != nullptr.
+// The CTC prefix beam search into nb (rows of nb.len_cap tokens) on `stream`, with workspace ws: zeroes every output
+// (token / time rows read 0 past a hypothesis' end, whatever the buffer held before), uploads the encoder lengths
+// through nb's host mirror, then searches, context-biased when graph != nullptr.
 static int prefix_beam_into(NBest& nb, const float* d_topk_val, const int* d_topk_idx, int k, const int* h_enc_lens,
                             int Tp, int blank_id, DevBuf& ws, ::rvb_context_graph* graph, cudaStream_t stream) {
   const NBest::Arrays d = nb.d(), h = nb.h();
   if (ws.ensure(prefix_beam_workspace_bytes(nb.B, Tp, nb.beam))) return -1;
+  RVB_CHECK_CUDA(cudaMemsetAsync(d.tim, 0, (size_t)(d.nhyp + nb.B - d.tim) * sizeof(int), stream));
   memcpy(h.lens, h_enc_lens, sizeof(int) * nb.B);
   RVB_CHECK_CUDA(cudaMemcpyAsync(d.lens, h.lens, sizeof(int) * nb.B, cudaMemcpyHostToDevice, stream));
   if (graph == nullptr)
@@ -1681,13 +1644,11 @@ static int rescoring_submit(rvb_model* m, SearchTicket& t, const float* h_cat, i
   t.h_r2l = nullptr;
   if (run_decoder) {
     RVB_REQUIRE(m->finalized && m->w.dec_l.present, "beam_search_rescoring: model has no decoder");
-    std::vector<float> cat_u;
     std::vector<int> grp;
     CatRows cr;
-    if (prepare_cat(m, true, h_cat, n_cat, B, &cat_u, &grp, &cr.G, stream)) return -1;
+    if (cat_rows(m, true, h_cat, n_cat, B, &cr, &grp, stream)) return -1;
     if (cr.G && upload_groups(grp, t.grp_pin, t.grp, stream)) return -1;
     cr.d_grp = t.grp.as<int>();
-    cr.st = &m->st_dec;
     const int Lp = Lmax + 1;
     const long long R = (long long)S * Lp;
     const bool use_r = reverse_weight > 0.f && m->w.dec_r.present && h_r2l != nullptr;
@@ -1802,8 +1763,8 @@ RVB_API int rvb_model_finalize(rvb_model* m) {
   return rvb::finalize_model(m);
 }
 
-// A second plan over the SAME packed weights with its own workspace (and its own folded language-specific
-// weights), so two host threads / CUDA streams can decode different batches concurrently.  The parent must outlive
+// A second plan over the SAME packed weights with its own workspace (and its own language-specific folds, made by its
+// calls), so two host threads / CUDA streams can decode different batches concurrently.  The parent must outlive
 // its forks.
 RVB_API rvb_model* rvb_model_fork(rvb_model* m) {
   if (m == nullptr || !m->finalized) {
@@ -1815,17 +1776,6 @@ RVB_API rvb_model* rvb_model_fork(rvb_model* m) {
   f->x3 = m->x3;
   f->finalized = true;
   f->w = m->w;
-  bool ok = true;
-  for (auto& E : f->w.enc)
-    if (E.lsl && rvb::alloc_fold(f, &E.lang)) ok = false;
-  for (rvb::Decoder* D : {&f->w.dec_l, &f->w.dec_r})
-    if (D->present)
-      for (auto& Ld : D->layers)
-        if (Ld.lsl && rvb::alloc_fold(f, &Ld.lang)) ok = false;
-  if (!ok) {
-    delete f;
-    return nullptr;
-  }
   return f;
 }
 
@@ -1944,9 +1894,7 @@ static int prefix_beam_search(const float* d_topk_val, const int* d_topk_idx, in
               "rvb_ctc_prefix_beam_search: bad arguments");
   rvb::NBest& nb = g_search_nb;
   if (nb.ensure(B, beam, max_len)) return -1;
-  const rvb::NBest::Arrays d = nb.d(), h = nb.h();
-  // zero every output (token / time rows read 0 past a hypothesis' end); the lens slot in between is uploaded after
-  RVB_CHECK_CUDA(cudaMemsetAsync(d.tim, 0, (size_t)(d.nhyp + B - d.tim) * sizeof(int), stream));
+  const rvb::NBest::Arrays h = nb.h();
   if (rvb::prefix_beam_into(nb, d_topk_val, d_topk_idx, k, h_enc_lens, Tp, blank_id, g_search_ws, graph, stream))
     return -1;
   RVB_CHECK_CUDA(cudaMemcpyAsync(nb.host.p, nb.dev.p, nb.bytes(), cudaMemcpyDeviceToHost, stream));

@@ -15,7 +15,8 @@ namespace rvb {
 inline std::atomic<long long> g_held_device{0}, g_held_pinned{0};
 
 // Grow-only buffer: ensure(n) keeps the allocation when it already holds n bytes, else replaces it by one of
-// n + n/8 + 256 bytes (device) or n + 256 bytes (page-locked host).  Move-only: the destructor frees.
+// n + n/8 + 256 bytes (device) or n + 256 bytes (page-locked host), or of exactly n bytes when `exact` (a buffer that
+// grows in rare, whole steps, such as a fold stack slot by slot).  Move-only: the destructor frees.
 template <bool Pinned>
 struct GrowBuf {
   void* p = nullptr;
@@ -38,10 +39,10 @@ struct GrowBuf {
     return *this;
   }
   ~GrowBuf() { release(); }
-  int ensure(size_t bytes) {
+  int ensure(size_t bytes, bool exact = false) {
     if (bytes <= cap) return 0;
     release();
-    const size_t want = Pinned ? bytes + 256 : bytes + (bytes >> 3) + 256;
+    const size_t want = exact ? bytes : Pinned ? bytes + 256 : bytes + (bytes >> 3) + 256;
     void* q = nullptr;
     RVB_CHECK_CUDA(Pinned ? cudaMallocHost(&q, want) : cudaMalloc(&q, want));
     p = q;
@@ -99,15 +100,6 @@ class WeightStore {
     void* p = nullptr;
     if (alloc(n * sizeof(T), &p)) return -1;
     RVB_CHECK_CUDA(cudaMemcpy(p, src, n * sizeof(T), cudaMemcpyHostToDevice));
-    *dst = reinterpret_cast<T*>(p);
-    return 0;
-  }
-  // n zeroed elements of T (and the pad bytes), owned by the store
-  template <typename T>
-  int alloc_zeroed(size_t n, T** dst) {
-    void* p = nullptr;
-    if (alloc(n * sizeof(T), &p)) return -1;
-    RVB_CHECK_CUDA(cudaMemset(p, 0, n * sizeof(T) + kPad));
     *dst = reinterpret_cast<T*>(p);
     return 0;
   }
