@@ -348,6 +348,38 @@ RVB_API int rvb_relpos_prep(const void* d_k, int ldk, const void* d_pos, int ldp
                             void* stream);
 RVB_API int rvb_f32_to_bf16(const float* d_x, void* d_out, long long n, void* stream);
 
+/* ---- FLAC decoding (RFC 9639; csrc/flac.cu, DESIGN.md §4k) ------------------------------------------------------
+ * The caller parses the metadata blocks on the host and uploads the whole file once (d_bytes, n_bytes); the frames
+ * start at byte audio_offset, right after the last metadata block.  rvb_flac_index finds the frames, rvb_flac_decode
+ * decodes them; both synchronise the stream before returning. */
+typedef struct rvb_flac_info {
+  int sample_rate;      /* STREAMINFO: Hz, > 0 */
+  int channels;         /* 1..8 */
+  int bits_per_sample;  /* 4..32 */
+  int max_block_size;   /* samples per channel of the largest frame (a launch-shape hint; larger frames still decode) */
+} rvb_flac_info;
+/* device workspace rvb_flac_index needs for a file of n_bytes bytes; it holds the frame index rvb_flac_decode reads */
+RVB_API long long rvb_flac_index_workspace_bytes(long long n_bytes);
+/* Finds every frame header (sync code, valid fields, CRC-8) and keeps the chain of frames whose coded frame / sample
+ * numbers are consecutive from the frame at audio_offset.  h_n_frames: frames in the chain, 0 when no valid frame
+ * header is at audio_offset, -1 when the bytes hold more sync candidates than any FLAC stream of that size;
+ * h_total_samples: their block sizes summed (STREAMINFO may state 0, "unknown"). */
+RVB_API int rvb_flac_index(const void* d_bytes, long long n_bytes, long long audio_offset, const rvb_flac_info* info,
+                           void* d_workspace, long long workspace_bytes, int* h_n_frames, long long* h_total_samples,
+                           void* stream);
+/* device workspace rvb_flac_decode needs; -1 on bad arguments */
+RVB_API long long rvb_flac_decode_workspace_bytes(int n_frames, long long total_samples, const rvb_flac_info* info);
+/* Decodes the indexed frames into d_out (channels, total_samples), left-justified: int16 (x << (16 - bps)) for
+ * bits_per_sample <= 16, int32 (x << (32 - bps)) above.  Every frame is checked (header against STREAMINFO, subframe
+ * syntax, bounds of every read, CRC-16, the frame ending where the next begins); h_bad_frame is the lowest failing frame
+ * (-1: none), h_bad_offset the byte offset concerned and h_bad_status its cause: 1 bad header, 2 header disagrees with
+ * STREAMINFO, 3 bad subframe, 4 bad residual coding, 5 frame truncated, 6 CRC-16 mismatch, 7 no frame header where the
+ * frame ends.  Samples of a failing frame are not written. */
+RVB_API int rvb_flac_decode(const void* d_bytes, long long n_bytes, const rvb_flac_info* info,
+                            const void* d_index_workspace, int n_frames, long long total_samples, void* d_workspace,
+                            long long workspace_bytes, void* d_out, int* h_bad_frame, long long* h_bad_offset,
+                            int* h_bad_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,6 +43,11 @@ class EmbConfig(C.Structure):
                 ("blocks", C.c_int * 4)]
 
 
+class FlacInfo(C.Structure):
+    """Mirror of `rvb_flac_info` (include/rvb_b200.h)."""
+    _fields_ = [(n, C.c_int) for n in ("sample_rate", "channels", "bits_per_sample", "max_block_size")]
+
+
 _vp, _i, _f, _ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
 
 # name -> (restype, argtypes); must list every symbol the header declares (tests/test_abi.py checks)
@@ -113,6 +118,10 @@ SIGNATURES = {
     "rvb_attention_tc_blocks_per_sm": (_i, [_i, _i, _i, _i]),
     "rvb_relpos_prep": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "rvb_f32_to_bf16": (_i, [_vp, _vp, _ll, _vp]),
+    "rvb_flac_index_workspace_bytes": (_ll, [_ll]),
+    "rvb_flac_index": (_i, [_vp, _ll, _ll, C.POINTER(FlacInfo), _vp, _ll, _vp, _vp, _vp]),
+    "rvb_flac_decode_workspace_bytes": (_ll, [_i, _ll, C.POINTER(FlacInfo)]),
+    "rvb_flac_decode": (_i, [_vp, _ll, C.POINTER(FlacInfo), _vp, _i, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp]),
     # include/rvb_diar.h
     "rvb_seg_create": (_vp, [C.POINTER(SegConfig)]),
     "rvb_seg_set_tensor": (_i, [_vp, C.c_char_p, _vp, _ll]),

@@ -15,7 +15,8 @@ from pathlib import Path
 def get_args(argv=None):
     p = argparse.ArgumentParser(description="Align a known transcript to a wav file with the Rev model (CTC forced alignment).")
     p.add_argument("--model", required=True, help="Path to a directory with config and checkpoint, or a pretrained model name")
-    p.add_argument("--audio_file", required=True, help="Audio the transcript belongs to")
+    p.add_argument("--audio_file", required=True, help="Audio the transcript belongs to (WAV or FLAC natively; other "
+                   "containers through torchaudio)")
     src = p.add_mutually_exclusive_group(required=True)
     src.add_argument("--text_file", help="Transcript as text (tokenised with the model's sentencepiece model)")
     src.add_argument("--token_file", help="Transcript as whitespace-separated token ids")

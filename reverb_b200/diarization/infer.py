@@ -48,11 +48,12 @@ def load_pipeline(model_dir: str = None, synthetic=False, device: int = 0, **kwa
     return SpeakerDiarization(segmentation_model(seg_sd, device=device), EmbeddingModel(emb_sd, device=device), **kwargs)
 
 
-def read_audio(path: str) -> np.ndarray:
-    """mono float32 in [-1, 1] at 16 kHz (pyannote's Audio(sample_rate=16000, mono="downmix"))"""
+def read_audio(path: str, device=None) -> np.ndarray:
+    """mono float32 in [-1, 1] at 16 kHz (pyannote's Audio(sample_rate=16000, mono="downmix")); FLAC frames are decoded
+    on `device` (default: the current device)"""
     from .. import _lib, audio_io
     from ..resample import resampled_length, sinc_resample_kernel
-    wav, sr = audio_io.load_audio(path)                           # (channels, samples), int16-valued or float
+    wav, sr = audio_io.load_audio(path, device)                   # (channels, samples), int16-valued or float
     integer_pcm = np.issubdtype(np.asarray(wav).dtype, np.integer)
     x = np.asarray(wav, np.float32)
     if x.ndim == 2:
@@ -73,7 +74,7 @@ def read_audio(path: str) -> np.ndarray:
 
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="Run speaker diarization on audio files")
-    ap.add_argument("audios", nargs="+")
+    ap.add_argument("audios", nargs="+", help="WAV or FLAC files (other containers need a torchaudio backend)")
     ap.add_argument("--out-dir", type=Path, required=True)
     ap.add_argument("--hf-access-token", type=str, default=None, help="accepted for CLI compatibility; unused offline")
     ap.add_argument("--pipeline-model", type=str, default=None, help="local directory with segmentation.pt / embedding.pt")
@@ -86,7 +87,7 @@ def main(argv=None) -> int:
     pipe = load_pipeline(args.pipeline_model, synthetic="v2" if args.synthetic_v2 else args.synthetic)
     for audio in args.audios:
         print("Processing", audio)
-        turns = pipe(read_audio(audio))
+        turns = pipe(read_audio(audio, pipe.segmentation.device))
         uri = os.path.splitext(os.path.basename(audio))[0]
         with open(args.out_dir / f"{uri}.rttm", "w") as f:
             pipe.write_rttm(f, uri, turns)

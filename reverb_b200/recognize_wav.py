@@ -20,7 +20,8 @@ def get_args(argv=None):
     from .reverb import get_available_models
     p = argparse.ArgumentParser(description="Run automatic speech recognition on a given wav file using the Rev model.")
     p.add_argument("--audio_file", required=True, nargs="+",
-                   help="Audio to transcribe; several files are decoded together, in shared batches")
+                   help="Audio to transcribe (WAV or FLAC natively; other containers through torchaudio); several "
+                        "files are decoded together, in shared batches")
     p.add_argument("--config", default=None, help="Path to config file")
     p.add_argument("--checkpoint", default=None, help="Path to Reverb model checkpoint")
     p.add_argument("--model", default=None,

@@ -43,10 +43,11 @@ CACHED_MODELS_DIR = Path.home() / ".cache/reverb"
 _MODELS = {"reverb_asr_v1": "https://huggingface.co/Revai/reverb-asr"}
 
 
-def _read_wav(path: str) -> Tuple[np.ndarray, int]:
-    """samples (channels, n) + sample rate — the `torchaudio.load(normalize=False)` contract (audio_io.py)."""
+def _read_wav(path: str, device=None) -> Tuple[np.ndarray, int]:
+    """samples (channels, n) + sample rate — the `torchaudio.load(normalize=False)` contract (audio_io.py); FLAC
+    frames are decoded on `device`."""
     from .audio_io import load_audio
-    return load_audio(path)
+    return load_audio(path, device)
 
 
 def _load_state_dict(checkpoint: str) -> Dict[str, torch.Tensor]:
@@ -137,7 +138,7 @@ class ReverbASR:
     def _read_recording(self, audio_file, resample_rate: int = 16000) -> "_Recording":
         """Reads channel 0 of a recording on the host.  Raises the front end's error for a recording that has fewer
         than 400 samples at `resample_rate`, before anything is uploaded."""
-        pcm, sample_rate = _read_wav(audio_file)
+        pcm, sample_rate = _read_wav(audio_file, self.device)
         logging.info(f"detected sample rate: {sample_rate}")
         ch0 = np.array(pcm[0], copy=True)                      # channel 0 (kaldi.fbank channel=-1 -> 0)
         if ch0.dtype != np.int16:
@@ -534,7 +535,8 @@ def speaker_outputs(diarization, audio_file, ctms: List[str]) -> Tuple[str, List
     from .diarization.infer import read_audio
     from .diarization.words2speakers import rttm_text, stm_text
     uri = os.path.splitext(os.path.basename(str(audio_file)))[0]
-    rttm = rttm_text(uri, diarization(read_audio(str(audio_file))))
+    device = getattr(getattr(diarization, "segmentation", None), "device", None)   # any callable diarizes
+    rttm = rttm_text(uri, diarization(read_audio(str(audio_file), device)))
     return rttm, [stm_text(uri, rttm, ctm) for ctm in ctms]
 
 
