@@ -380,6 +380,24 @@ RVB_API int rvb_flac_decode(const void* d_bytes, long long n_bytes, const rvb_fl
                             long long workspace_bytes, void* d_out, int* h_bad_frame, long long* h_bad_offset,
                             int* h_bad_status, void* stream);
 
+/* ---- compressed WAV decoding: G.711 and ADPCM (csrc/wav_codec.cu, DESIGN.md §4l) ---------------------------------
+ * The caller parses and validates the fmt chunk on the host and uploads the data chunk once (d_data, n_bytes). */
+typedef struct rvb_wav_codec {
+  int format_tag;         /* WAVE format tag: 0x0007 mu-law, 0x0006 A-law, 0x0011 IMA ADPCM, 0x0002 MS ADPCM */
+  int channels;           /* >= 1 (MS ADPCM: 1 or 2) */
+  int block_align;        /* bytes per block; G.711: channels */
+  int samples_per_block;  /* per channel, header samples included (ADPCM) */
+  int n_coef;             /* MS ADPCM: coefficient pairs, 7..256 */
+  short coef[512];        /* MS ADPCM: n_coef pairs (c1, c2) */
+} rvb_wav_codec;
+/* Decodes the first `frames` samples of every channel into d_out (channels, frames) int16; samples past `frames` are
+ * not written and no read leaves its block or the data span.  G.711 expands every byte; an ADPCM block decodes from
+ * the state in its header, one thread per (block, channel).  h_bad_block is the lowest block whose header is invalid
+ * (-1: none) and h_bad_status its cause: 1 IMA step index above 88, 2 MS ADPCM predictor index >= n_coef.  Returns -2
+ * when `frames` is more than the bytes hold.  Synchronises the stream before returning. */
+RVB_API int rvb_wav_decode(const void* d_data, long long n_bytes, const rvb_wav_codec* info, long long frames,
+                           void* d_out, int* h_bad_block, int* h_bad_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -48,6 +48,12 @@ class FlacInfo(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("sample_rate", "channels", "bits_per_sample", "max_block_size")]
 
 
+class WavCodec(C.Structure):
+    """Mirror of `rvb_wav_codec` (include/rvb_b200.h)."""
+    _fields_ = [(n, C.c_int) for n in ("format_tag", "channels", "block_align", "samples_per_block", "n_coef")] + \
+               [("coef", C.c_short * 512)]
+
+
 _vp, _i, _f, _ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
 
 # name -> (restype, argtypes); must list every symbol the header declares (tests/test_abi.py checks)
@@ -122,6 +128,7 @@ SIGNATURES = {
     "rvb_flac_index": (_i, [_vp, _ll, _ll, C.POINTER(FlacInfo), _vp, _ll, _vp, _vp, _vp]),
     "rvb_flac_decode_workspace_bytes": (_ll, [_i, _ll, C.POINTER(FlacInfo)]),
     "rvb_flac_decode": (_i, [_vp, _ll, C.POINTER(FlacInfo), _vp, _i, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp]),
+    "rvb_wav_decode": (_i, [_vp, _ll, C.POINTER(WavCodec), _ll, _vp, _vp, _vp, _vp]),
     # include/rvb_diar.h
     "rvb_seg_create": (_vp, [C.POINTER(SegConfig)]),
     "rvb_seg_set_tensor": (_i, [_vp, C.c_char_p, _vp, _ll]),

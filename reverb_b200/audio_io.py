@@ -7,6 +7,10 @@ RIFF/WAVE is parsed here (PCM 8 / 16 / 24 / 32 bit, IEEE float 32 / 64, WAVE_FOR
 the stdlib `wave` module only does plain PCM.  Value conventions follow torchaudio: uint8 stays unsigned 0..255,
 24-bit samples are left-justified in int32 (x << 8), 32-bit stay int32, float64 is narrowed to float32.
 
+G.711 µ-law / A-law and IMA / Microsoft ADPCM WAV (format tags 0x0007, 0x0006, 0x0011, 0x0002; G.711 also inside
+WAVE_FORMAT_EXTENSIBLE) are validated here and decoded on the GPU (csrc/wav_codec.cu, DESIGN.md §4l) to int16, what
+torchaudio 2.2's FFmpeg backend returns for them with normalize=False.
+
 FLAC (detected by its `fLaC` magic, optionally behind an ID3v2 tag, whatever the file is called) is decoded natively:
 the metadata blocks are parsed here on the host and the frames are decoded on the GPU (csrc/flac.cu, DESIGN.md §4k).
 Samples come back as integers, left-justified like the WAV path's: int16 (x << (16 - bps)) for up to 16 bits per
@@ -29,12 +33,21 @@ from typing import List, Tuple
 import numpy as np
 
 WAVE_FORMAT_PCM, WAVE_FORMAT_IEEE_FLOAT, WAVE_FORMAT_EXTENSIBLE = 0x0001, 0x0003, 0xFFFE
+WAVE_FORMAT_ADPCM, WAVE_FORMAT_ALAW, WAVE_FORMAT_MULAW, WAVE_FORMAT_IMA_ADPCM = 0x0002, 0x0006, 0x0007, 0x0011
+# WAVE format tags decoded on the GPU (csrc/wav_codec.cu, DESIGN.md §4l) -> codec name used in error messages
+WAV_CODECS = {WAVE_FORMAT_MULAW: "G.711 mu-law", WAVE_FORMAT_ALAW: "G.711 A-law", WAVE_FORMAT_IMA_ADPCM: "IMA ADPCM",
+              WAVE_FORMAT_ADPCM: "MS ADPCM"}
+# the seven coefficient pairs every MS ADPCM file starts its table with
+MS_ADPCM_COEFS = ((256, 0), (512, -256), (0, 0), (192, 64), (240, 0), (460, -208), (392, -232))
+# rvb_wav_decode's status codes (include/rvb_b200.h)
+_WAV_CODEC_STATUS = {1: "IMA ADPCM step index above 88", 2: "MS ADPCM predictor index beyond the coefficient table"}
 
 
-def _parse_riff_wave(data: bytes, path: str) -> Tuple[np.ndarray, int]:
+def _parse_riff_wave(data: bytes, path: str, device=None) -> Tuple[np.ndarray, int]:
     if len(data) < 12 or data[:4] != b"RIFF" or data[8:12] != b"WAVE":
         raise ValueError(f"{path}: not a RIFF/WAVE file")
     pos, fmt, pcm = 12, None, None
+    fmt_body, data_off, fact = b"", 0, None
     while pos + 8 <= len(data):
         cid, size = data[pos:pos + 4], struct.unpack_from("<I", data, pos + 4)[0]
         body = data[pos + 8:pos + 8 + size]
@@ -44,17 +57,26 @@ def _parse_riff_wave(data: bytes, path: str) -> Tuple[np.ndarray, int]:
             tag, nch, rate, _brate, block, bits = struct.unpack_from("<HHIIHH", body, 0)
             if tag == WAVE_FORMAT_EXTENSIBLE and len(body) >= 40:
                 tag = struct.unpack_from("<H", body, 24)[0]          # first two bytes of the SubFormat GUID
+                if tag in (WAVE_FORMAT_ADPCM, WAVE_FORMAT_IMA_ADPCM):  # its extension is not the ADPCM one
+                    raise ValueError(f"{path}: unsupported WAVE format tag 0x{tag:04x} inside WAVE_FORMAT_EXTENSIBLE")
             fmt = (tag, nch, rate, block, bits)
+            fmt_body = body
         elif cid == b"data":
             pcm = body                                               # a streamed file may state size 0xFFFFFFFF: slice clips
+            data_off = pos + 8
+        elif cid == b"fact" and len(body) >= 4:
+            fact = struct.unpack_from("<I", body, 0)[0]              # dwSampleLength: frames per channel
         pos += 8 + size + (size & 1)                                 # chunks are word aligned
     if fmt is None or pcm is None:
         raise ValueError(f"{path}: missing fmt or data chunk")
     tag, nch, rate, block, bits = fmt
     if nch < 1:
         raise ValueError(f"{path}: bad channel count {nch}")
+    if tag in WAV_CODECS:
+        return _decode_wav_codec(pcm, fmt, fmt_body, fact, data_off, path, device), int(rate)
     if tag not in (WAVE_FORMAT_PCM, WAVE_FORMAT_IEEE_FLOAT):
-        raise ValueError(f"{path}: unsupported WAVE format tag 0x{tag:04x} (only PCM and IEEE float)")
+        raise ValueError(f"{path}: unsupported WAVE format tag 0x{tag:04x} (PCM, IEEE float, G.711 mu-law / A-law, "
+                         "IMA ADPCM and MS ADPCM are decoded)")
     if bits % 8 != 0 or bits == 0:
         raise ValueError(f"{path}: unsupported sample width {bits}")
     width = bits // 8
@@ -81,6 +103,109 @@ def _parse_riff_wave(data: bytes, path: str) -> Tuple[np.ndarray, int]:
         else:
             raise ValueError(f"{path}: unsupported float width {bits}")
     return np.ascontiguousarray(x.reshape(nfr, nch).T), int(rate)
+
+
+@dataclass
+class WavCodecInfo:
+    """A validated compressed-WAV fmt chunk and the frame count its data chunk decodes to."""
+    format_tag: int
+    channels: int
+    block_align: int
+    samples_per_block: int                 # per channel, ADPCM; 1 for G.711
+    coefs: List[Tuple[int, int]]           # MS ADPCM coefficient pairs
+    frames: int                            # per channel
+
+
+def parse_wav_codec(pcm: bytes, fmt, fmt_body: bytes, fact, data_off: int, path: str = "<bytes>") -> WavCodecInfo:
+    """Validates the fmt chunk of a G.711 or ADPCM WAV and counts its frames: G.711 has one byte per sample; an ADPCM
+    data chunk is full blocks then an optional partial block, and a `fact` chunk, when present, states the length.
+    Every error is a ValueError naming the file, the format tag and the codec; nothing here touches the GPU."""
+    tag, nch, _rate, block, bits = fmt
+    codec = WAV_CODECS[tag]
+
+    def bad(msg):
+        return ValueError(f"{path}: format tag 0x{tag:04x} ({codec}): {msg}")
+    cb = struct.unpack_from("<H", fmt_body, 16)[0] if len(fmt_body) >= 18 else 0
+    if tag in (WAVE_FORMAT_MULAW, WAVE_FORMAT_ALAW):
+        if bits != 8:
+            raise bad(f"{bits} bits per sample (G.711 has 8)")
+        if block != nch:
+            raise bad(f"block_align {block} for {nch} channels (must equal the channel count)")
+        return WavCodecInfo(tag, nch, block, 1, [], len(pcm) // nch)
+    if bits != 4:
+        raise bad(f"{bits} bits per sample (only 4-bit ADPCM is decoded)")
+    if tag == WAVE_FORMAT_IMA_ADPCM:
+        if cb < 2:
+            raise bad(f"fmt extension of {cb} bytes (cbSize must be at least 2, for wSamplesPerBlock)")
+        spb = struct.unpack_from("<H", fmt_body, 18)[0]
+        if spb < 1 or (spb - 1) % 8:
+            raise bad(f"{spb} samples per block (must be 1 + a multiple of 8)")
+        if block != 4 * nch * (1 + (spb - 1) // 8):
+            raise bad(f"block_align {block} does not hold {spb} samples of {nch} channels "
+                      f"(expected {4 * nch * (1 + (spb - 1) // 8)})")
+        hdr, coefs = 4 * nch, []
+    else:
+        if nch not in (1, 2):
+            raise bad(f"{nch} channels (MS ADPCM has 1 or 2)")
+        if cb < 32 or len(fmt_body) < 22:
+            raise bad(f"fmt extension of {cb} bytes (cbSize must be at least 32, for the coefficient table)")
+        spb, n_coef = struct.unpack_from("<HH", fmt_body, 18)
+        if not 7 <= n_coef <= 256:
+            raise bad(f"{n_coef} coefficient pairs (7 to 256 are valid)")
+        if len(fmt_body) < 22 + 4 * n_coef or cb < 4 + 4 * n_coef:
+            raise bad(f"fmt chunk too short for its {n_coef} coefficient pairs")
+        coefs = [struct.unpack_from("<hh", fmt_body, 22 + 4 * i) for i in range(n_coef)]
+        if tuple(coefs[:7]) != MS_ADPCM_COEFS:
+            raise bad(f"the first seven coefficient pairs {coefs[:7]} are not the standard table")
+        if block < 7 * nch or spb != 2 + (block - 7 * nch) * 2 // nch:
+            raise bad(f"{spb} samples per block do not fit block_align {block} for {nch} channels")
+        hdr = 7 * nch
+    full, rem = divmod(len(pcm), block)
+    part = 0
+    if rem:
+        if rem < hdr:
+            raise bad(f"block {full} at byte {data_off + full * block}: truncated: {rem} bytes, its header needs {hdr}")
+        part = 1 + 8 * ((rem - hdr) // hdr) if tag == WAVE_FORMAT_IMA_ADPCM else 2 + (rem - hdr) * 2 // nch
+    frames = full * spb + part
+    if fact is not None:
+        if fact > frames:
+            k = frames // spb
+            raise bad(f"block {k} at byte {data_off + k * block}: missing: the data chunk holds {frames} samples per "
+                      f"channel in {full + (1 if rem else 0)} blocks, the fact chunk states {fact}")
+        frames = fact
+    return WavCodecInfo(tag, nch, block, spb, coefs, frames)
+
+
+def _decode_wav_codec(pcm: bytes, fmt, fmt_body: bytes, fact, data_off: int, path: str, device) -> np.ndarray:
+    import torch
+
+    from . import _lib
+    wi = parse_wav_codec(pcm, fmt, fmt_body, fact, data_off, path)
+    if wi.frames == 0:
+        return np.zeros((wi.channels, 0), np.int16)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"{path}: {WAV_CODECS[wi.format_tag]} WAV is decoded on the GPU and no CUDA device is "
+                           "available (reverb_b200 has no CPU fallback)")
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    lib = _lib.load()
+    info = _lib.WavCodec(wi.format_tag, wi.channels, wi.block_align, wi.samples_per_block, len(wi.coefs))
+    for i, (c1, c2) in enumerate(wi.coefs):
+        info.coef[2 * i], info.coef[2 * i + 1] = c1, c2
+    bad_block, bad_status = ctypes.c_int(-1), ctypes.c_int(0)
+    # a stream of its own, as for FLAC: the reader thread decodes while the caller's stream runs the model
+    stream = torch.cuda.Stream(device=dev)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        d_bytes = torch.frombuffer(bytearray(pcm), dtype=torch.uint8).to(dev)
+        out = torch.empty((wi.channels, wi.frames), dtype=torch.int16, device=dev)
+        _lib.check(lib.rvb_wav_decode(d_bytes.data_ptr(), len(pcm), ctypes.byref(info), wi.frames, out.data_ptr(),
+                                      ctypes.byref(bad_block), ctypes.byref(bad_status), stream.cuda_stream),
+                   "rvb_wav_decode")
+        if bad_block.value >= 0:
+            k = bad_block.value
+            raise ValueError(f"{path}: format tag 0x{wi.format_tag:04x} ({WAV_CODECS[wi.format_tag]}): block {k} at "
+                             f"byte {data_off + k * wi.block_align}: "
+                             f"{_WAV_CODEC_STATUS.get(bad_status.value, f'status {bad_status.value}')}")
+        return out.cpu().numpy()
 
 
 FLAC_BLOCK_TYPES = {0: "STREAMINFO", 1: "PADDING", 2: "APPLICATION", 3: "SEEKTABLE", 4: "VORBIS_COMMENT", 5: "CUESHEET",
@@ -204,11 +329,12 @@ def _decode_flac(data: bytes, path: str, device) -> Tuple[np.ndarray, int]:
 
 def load_audio(path: str, device=None) -> Tuple[np.ndarray, int]:
     """(channels, frames) samples + sample rate, `torchaudio.load(path, normalize=False)` semantics.
-    device: the CUDA device FLAC frames are decoded on (default: the current device); WAV never touches the GPU."""
+    device: the CUDA device FLAC frames and G.711 / ADPCM WAV data are decoded on (default: the current device); PCM
+    and float WAV never touch the GPU."""
     with open(path, "rb") as f:
         head = f.read(12)
         if head[:4] == b"RIFF" and head[8:12] == b"WAVE":
-            return _parse_riff_wave(head + f.read(), str(path))
+            return _parse_riff_wave(head + f.read(), str(path), device)
         skip = _id3v2_size(head[:10])
         if skip:
             f.seek(skip)
