@@ -16,6 +16,10 @@
 //                    (bias / ReLU / SiLU / GLU / residual(+row mask) / log-sum-exp / rel-pos keys) on a shared-memory
 //                    copy of the accumulator; outputs pass through a per-warp XOR-swizzled staging tile so global
 //                    accesses are coalesced.
+// Wide bf16-output layers (bias / ReLU / SiLU, N % 256 == 0, at least one wave of tiles: FFN1, the conv2 implicit GEMM)
+// run on 128 x 256 tiles instead (gemm_wide_kernel): both consumer warpgroups share one tile and one 256-wide weight
+// tile per k-block, and the producer warpgroup's idle warps store the bf16 output tile.  RVB_GEMM_WIDE=0 (read per
+// call) keeps them on 128 x 128 tiles; the outputs are the same bits.
 // Tuning aid (environment, read once): RVB_GEMM_SKIP_EPI=1|2|3 (main loop only / no global stores / accumulator
 // reads + math only — results are wrong by construction; tools/gemm_bench.py).  RVB_GEMM=simt selects the CUDA-core
 // bring-up kernel, RVB_GEMM=narrow 64-wide tiles wherever the epilogue allows them.
@@ -898,6 +902,176 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// 128 x 256 tiles for the wide bf16-output GEMMs (FFN1, the conv2 implicit GEMM, ...).  3 stages of 48 KB + the 64 KB
+// bf16 output tile = 208 KB; a 4th stage does not fit beside the output tile.
+struct WideCfg {
+  static constexpr int BM = 128;
+  static constexpr int BN = 256;
+  static constexpr int BK = 64;
+  static constexpr int STAGES = 3;
+  static constexpr uint32_t A_BYTES = BM * BK * 2;
+  static constexpr uint32_t B_BYTES = BN * BK * 2;
+  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr uint32_t OUT_BYTES = BM * BN * 2;
+  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + OUT_BYTES + 256 /*barriers*/ + 1024 /*align slack*/;
+};
+
+// Persistent TMA + wgmma GEMM on 128 x 256 tiles for the bf16-output epilogues without cross-column work (bias, ReLU,
+// SiLU; EPI_BF16 / EPI_BF16_RELU / EPI_BF16_SILU, plain or conv_mode, no hi/lo pair).  Per k-block the SM pulls one
+// 256-wide weight tile that both consumer warpgroups read: 48 KB per 4.2 MFLOP instead of 32 KB per 2.1 MFLOP.
+//   warpgroup 0, warp 0 : TMA producer (one thread) — a 3-deep ring of {A 128x64, W 256x64} bf16 tiles (SWIZZLE_128B)
+//   warpgroup 0, warps 1-3 : copy the bf16 output tile from shared memory to global memory (16-byte stores, one
+//                    512-byte row per warp instruction) under the next tile's main loop
+//   warpgroups 1-2 : consumers of the same tile, rows 0-63 and 64-127: wgmma m64n256k16 x 4 per k-block (the k order of
+//                    gemm_wg_kernel), each stage released once all 8 consumer warps have retired their MMAs.  Then bias
+//                    and activation in registers, with gemm_wg_kernel's arithmetic, into the bf16 output tile.
+// One mbarrier pair guards the output tile:
+//   ofull : arrived by the 256 consumer threads once tile i is written — the copy warps may read it;
+//   ofree : arrived by the 96 copy threads once tile i is stored — the consumers may write tile i + 1.
+// Each completes once per tile, so the CTA's tile i waits for completion i + 1 of ofull (parity i & 1), and tile i
+// (i >= 1) waits for completion i of ofree (parity (i - 1) & 1); tile 0 writes without waiting.  A barrier is never
+// more than one phase ahead of its waiter: ofull's next arrivals need ofree's previous completion and vice versa.
+// RVB_GEMM_SKIP_EPI=1 skips the epilogue (main loop only), 2 the global stores; the barrier hand-offs stay.
+template <int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
+  using Cfg = WideCfg;
+  constexpr int STAGES = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
+  uint8_t* sOut = smem + STAGES * Cfg::STAGE_BYTES;   // bf16 [128][256], 16-byte chunk c of row r at c ^ (r % 8)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + Cfg::OUT_BYTES);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + STAGES;
+  uint64_t* ofull = bars + 2 * STAGES;
+  uint64_t* ofree = ofull + 1;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);   // lane 0 of every consumer warp
+    }
+    mbar_init(ofull, 256);
+    mbar_init(ofree, 96);
+    fence_barrier_init();
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+  }
+  __syncthreads();
+  const int nkb = p.num_k_blocks;
+
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0) {
+      // ---------------------------------------------------------- TMA producer
+      if (lane == 0) {
+        uint32_t stage = 0, phase = 0;
+        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+          const TileCoord t = decode_tile(p, tile, Cfg::BN);
+          for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+            if (p.conv_mode) {
+              const int tap = kb / p.conv_cblocks;
+              const int cb = kb - tap * p.conv_cblocks;
+              const int kh = tap / 3, kw = tap - kh * 3;
+              tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], cb * 64, 2 * t.f + kw, t.row0 + (kh >> 1),
+                          t.b * 2 + (kh & 1));
+            } else {
+              tma_load_4d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kb * 64, t.row0, 0, 0);
+            }
+            tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kb * 64, t.n0);
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+      }
+    } else {
+      // ---------------------------------------------------------- output tile -> global memory (warps 1-3)
+      const int cw = warp - 1;
+      const bool store = p.debug_skip_epi == 0;
+      bf16* out = reinterpret_cast<bf16*>(p.out);
+      int i = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
+        const TileCoord t = decode_tile(p, tile, Cfg::BN);
+        mbar_wait(ofull, i & 1);
+        if (store) {
+#pragma unroll 4
+          for (int r = cw; r < Cfg::BM; r += 3) {
+            const long long orow = output_row(p, t, r);
+            const uint4 u = *reinterpret_cast<const uint4*>(sOut + r * (Cfg::BN * 2) + ((lane ^ (r & 7)) << 4));
+            if (orow >= 0) *reinterpret_cast<uint4*>(out + orow * p.ldo + t.n0 + lane * 8) = u;
+          }
+        }
+        mbar_arrive(ofree);
+      }
+    }
+  } else {
+    // ------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    float acc[Cfg::BN / 2];   // rows 64 wg + [0, 64) of the tile (wgmma fragment layout, common.cuh)
+    uint32_t stage = 0, phase = 0;
+    int i = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
+      const TileCoord t = decode_tile(p, tile, Cfg::BN);
+#pragma unroll
+      for (int e = 0; e < Cfg::BN / 2; ++e) acc[e] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        constexpr uint64_t kHalfA = (Cfg::A_BYTES / 2) >> 4;   // rows 64-127 of the A stage, in descriptor units
+        const uint64_t adesc = make_sw128_desc(smem_u32(sA + stage * Cfg::A_BYTES)) + wg * kHalfA;
+        const uint64_t bdesc = make_sw128_desc(smem_u32(sB + stage * Cfg::B_BYTES));
+        wgmma_fence_regs<Cfg::BN / 2>(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n256k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous stage's MMAs have retired: release it
+        wgmma_fence_regs<Cfg::BN / 2>(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = (int)stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs<Cfg::BN / 2>(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      if (i > 0) mbar_wait(ofree, (i - 1) & 1);
+      if (p.debug_skip_epi != 1) {
+        // thread (wl, lane) holds rows r0 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1}; the 4 lanes of a row fill
+        // one 16-byte chunk, and the 8 rows of a warp store land in 8 distinct chunk slots (conflict-free)
+        const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+        uint32_t* so = reinterpret_cast<uint32_t*>(sOut) + r0 * (Cfg::BN / 2) + (lane & 3);
+        const float2 one2 = make_float2(1.f, 1.f);
+#pragma unroll
+        for (int j = 0; j < Cfg::BN / 8; ++j) {
+          float2 b = make_float2(0.f, 0.f);
+          if (p.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias + t.n0 + 8 * j + 2 * (lane & 3)));
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float2 v = ffma2(make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), one2, b);
+            if (EPI == EPI_BF16_SILU) v = gated2(v, v);
+            if (EPI == EPI_BF16_RELU) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+            so[8 * e * (Cfg::BN / 2) + ((j ^ (lane >> 2)) << 2)] = pack_bf16x2(v.x, v.y);
+          }
+        }
+      }
+      mbar_arrive(ofull);
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Debug / bring-up kernel: same contract on plain CUDA cores (RVB_GEMM=simt).  Never used by the benchmarks.
 __device__ __forceinline__ float load_a_elem(const GemmKParams& p, const TileCoord& t, int r, int k) {
@@ -1078,9 +1252,10 @@ int gemm_profile_end(double* total_ms, double* total_flops, long long* launches)
   return 0;
 }
 
+// BN = 256: gemm_wide_kernel (launch_gemm has checked that the epilogue is one it covers)
 template <int BN>
 static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  constexpr uint32_t SMEM_BYTES = BN == 256 ? WideCfg::SMEM_BYTES : GemmCfg<BN>::SMEM_BYTES;
   CUtensorMap tmA, tmB;
   const int kmul = a.x3 ? 2 : 1;
   const long long lda = a.lda ? a.lda : (long long)a.K * kmul, ldw = a.ldw ? a.ldw : (long long)a.K * kmul;
@@ -1103,20 +1278,28 @@ static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
     if (make_tmap(&tmB, a.W, 2, dims, str, box)) return -1;
   }
   void (*kern)(const CUtensorMap, const CUtensorMap, const GemmKParams) = nullptr;
-  const bool pair = a.out_split > 0;
-  switch (a.rp_pos ? (int)EPI_BF16_RELPOS : select_epi(a.act, a.out_mode)) {
-    case EPI_BF16: kern = pair ? gemm_wg_kernel<BN, EPI_BF16, true> : gemm_wg_kernel<BN, EPI_BF16, false>; break;
-    case EPI_BF16_RELU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_RELU, true> : gemm_wg_kernel<BN, EPI_BF16_RELU, false>; break;
-    case EPI_BF16_SILU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_SILU, true> : gemm_wg_kernel<BN, EPI_BF16_SILU, false>; break;
-    case EPI_F32: kern = gemm_wg_kernel<BN, EPI_F32, false>; break;
-    case EPI_RESID: kern = gemm_wg_kernel<BN, EPI_RESID, false>; break;
-    case EPI_GLU: kern = pair ? gemm_wg_kernel<BN, EPI_GLU, true> : gemm_wg_kernel<BN, EPI_GLU, false>; break;
-    case EPI_LSE: kern = gemm_wg_kernel<BN, EPI_LSE, false>; break;
-    case EPI_BF16_RELPOS: kern = gemm_wg_kernel<BN, EPI_BF16_RELPOS, false>; break;
-    case EPI_BF16_GELU: kern = gemm_wg_kernel<BN, EPI_BF16_GELU, false>; break;
-    default: kern = gemm_wg_kernel<BN, EPI_GENERIC, false>; break;
+  if constexpr (BN == 256) {
+    switch (select_epi(a.act, a.out_mode)) {
+      case EPI_BF16: kern = gemm_wide_kernel<EPI_BF16>; break;
+      case EPI_BF16_RELU: kern = gemm_wide_kernel<EPI_BF16_RELU>; break;
+      default: kern = gemm_wide_kernel<EPI_BF16_SILU>; break;
+    }
+  } else {
+    const bool pair = a.out_split > 0;
+    switch (a.rp_pos ? (int)EPI_BF16_RELPOS : select_epi(a.act, a.out_mode)) {
+      case EPI_BF16: kern = pair ? gemm_wg_kernel<BN, EPI_BF16, true> : gemm_wg_kernel<BN, EPI_BF16, false>; break;
+      case EPI_BF16_RELU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_RELU, true> : gemm_wg_kernel<BN, EPI_BF16_RELU, false>; break;
+      case EPI_BF16_SILU: kern = pair ? gemm_wg_kernel<BN, EPI_BF16_SILU, true> : gemm_wg_kernel<BN, EPI_BF16_SILU, false>; break;
+      case EPI_F32: kern = gemm_wg_kernel<BN, EPI_F32, false>; break;
+      case EPI_RESID: kern = gemm_wg_kernel<BN, EPI_RESID, false>; break;
+      case EPI_GLU: kern = pair ? gemm_wg_kernel<BN, EPI_GLU, true> : gemm_wg_kernel<BN, EPI_GLU, false>; break;
+      case EPI_LSE: kern = gemm_wg_kernel<BN, EPI_LSE, false>; break;
+      case EPI_BF16_RELPOS: kern = gemm_wg_kernel<BN, EPI_BF16_RELPOS, false>; break;
+      case EPI_BF16_GELU: kern = gemm_wg_kernel<BN, EPI_BF16_GELU, false>; break;
+      default: kern = gemm_wg_kernel<BN, EPI_GENERIC, false>; break;
+    }
   }
-  RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM_BYTES));
+  RVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   p.tiles_n = a.grp ? p.grp_slots * (p.group_n / BN) : (a.N + BN - 1) / BN;
   int tiles_m = a.conv_mode ? a.conv_B * a.conv_F2 * p.conv_tt : (a.M + 127) / 128;
   p.num_tiles = tiles_m * p.tiles_n;
@@ -1127,7 +1310,7 @@ static int launch_wg(const GemmArgs& a, GemmKParams& p, cudaStream_t stream) {
     rec.flops = 2.0 * (double)a.M * (double)(a.grp ? a.group_n : a.N) * (double)a.K * (a.x3 ? 3.0 : 1.0);
     RVB_CHECK_CUDA(cudaEventRecord(rec.a, stream));
   }
-  kern<<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  kern<<<grid, kGemmThreads, SMEM_BYTES, stream>>>(tmA, tmB, p);
   RVB_COUNT_LAUNCH();
   RVB_CHECK_LAUNCH();
   if (g_prof_on) {
@@ -1277,8 +1460,17 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   const bool narrow = p.group_n <= 64 || (get_gemm_impl() == 2 && a.out_mode != OUT_LSE && !(a.act == ACT_GLU && a.out_split > 0));
   RVB_REQUIRE(!a.grp || p.group_n % (narrow ? 64 : 128) == 0, "gemm: grouped output needs group_n %% %d == 0 (group_n=%d)",
               narrow ? 64 : 128, p.group_n);
-  if (!narrow) return launch_wg<128>(a, p, stream);
-  return launch_wg<64>(a, p, stream);
+  if (narrow) return launch_wg<64>(a, p, stream);
+  // 128 x 256 tiles (gemm_wide_kernel) for a plain bf16 output with bias / ReLU / SiLU, N % 256 == 0 and at least one
+  // wave of tiles; RVB_GEMM_WIDE=0 (read per call, so one process can A/B both) keeps every shape on 128 x 128 tiles
+  const int epi = select_epi(a.act, a.out_mode);
+  const long long wide_tiles = (long long)(a.conv_mode ? a.conv_B * a.conv_F2 * p.conv_tt : (a.M + 127) / 128) * (a.N / 256);
+  const char* wide_env = getenv("RVB_GEMM_WIDE");
+  if ((epi == EPI_BF16 || epi == EPI_BF16_RELU || epi == EPI_BF16_SILU) && !a.rp_pos && !a.grp && !a.x3 &&
+      a.out_split == 0 && p.bf16_coalesced && a.N % 256 == 0 && wide_tiles >= g_num_sms &&
+      !(wide_env && strcmp(wide_env, "0") == 0))
+    return launch_wg<256>(a, p, stream);
+  return launch_wg<128>(a, p, stream);
 }
 
 }  // namespace rvb

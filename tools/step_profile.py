@@ -4,7 +4,8 @@ per-kernel totals (launches, total ms, ms per step, share of the step) as JSON t
 a summary with the card's name and power limit.  The step time that the shares refer to is taken first, from CUDA
 events with the profiler off; the profiled steps run separately.
 
-`gemm_wg_kernel<BN, EPI, PAIR>` instantiations are labelled by the layer their epilogue serves (csrc/gemm.cu `Epi`).
+`gemm_wg_kernel<BN, EPI, PAIR>` and `gemm_wide_kernel<EPI>` instantiations are labelled by the layer their epilogue
+serves (csrc/gemm.cu `Epi`).
 
     python tools/step_profile.py OUT_DIR [--steps 3] [--warmup 3] [--chunks 64]
 """
@@ -24,6 +25,7 @@ GEMM_LAYERS = {0: "bf16 (embed / decoder)", 1: "conv2 (implicit GEMM, ReLU)", 2:
                3: "fp32 out", 4: "residual (FFN2, attn out, pointwise conv2)", 5: "generic",
                6: "pointwise conv1 (GLU)", 7: "CTC / decoder head (log-sum-exp)", 8: "QKV + rel-pos keys"}
 _GEMM_RE = re.compile(r"gemm_wg_kernel<(\d+),\s*(\d+),\s*(true|false)>")
+_WIDE_RE = re.compile(r"gemm_wide_kernel<(\d+)>")
 
 
 def card():
@@ -33,6 +35,9 @@ def card():
 
 
 def label(name):
+    w = _WIDE_RE.search(name)
+    if w:
+        return f"gemm_wide_kernel<{w.group(1)}> {GEMM_LAYERS.get(int(w.group(1)), '?')}"
     m = _GEMM_RE.search(name)
     if not m:
         return name
@@ -95,15 +100,15 @@ def main():
         kernels.append({"kernel": name, "count": d["count"], "total_ms": round(d["total_ms"], 3),
                         "ms_per_step": round(ms, 3), "share_of_step": round(ms / step_ms, 4)})
     kernels.sort(key=lambda k: -k["total_ms"])
-    gemm_ms = sum(k["ms_per_step"] for k in kernels if k["kernel"].startswith("gemm_wg_kernel"))
+    gemm_ms = sum(k["ms_per_step"] for k in kernels if k["kernel"].startswith(("gemm_wg_kernel", "gemm_wide_kernel")))
     out = {"card": card(), "lib": os.environ.get("RVB_LIB_PATH") or "in-tree", "chunks": args.chunks,
            "profiled_steps": args.steps, "step_ms_unprofiled": round(step_ms, 3),
-           "gemm_wg_kernel_ms_per_step": round(gemm_ms, 3),
+           "gemm_ms_per_step": round(gemm_ms, 3),
            "all_kernels_ms_per_step": round(sum(k["ms_per_step"] for k in kernels), 3), "kernels": kernels}
     path = os.path.join(args.out_dir, "step_profile.json")
     with open(path, "w") as f:
         json.dump(out, f, indent=1)
-    print(f"{out['card']}: step {step_ms:.2f} ms (profiler off), gemm_wg_kernel {gemm_ms:.2f} ms/step -> {path}")
+    print(f"{out['card']}: step {step_ms:.2f} ms (profiler off), GEMM kernels {gemm_ms:.2f} ms/step -> {path}")
     for k in kernels[:25]:
         print(f"  {k['ms_per_step']:9.3f} ms/step {100 * k['share_of_step']:5.1f} %  x{k['count']:<5d} {k['kernel'][:110]}")
 
